@@ -441,7 +441,7 @@ int ordinals_launch(const agb_desc &d, Workspace &W, const void *d_text, uint64_
 	else { k_delim_count<<<(unsigned)tiles, ORD_THREADS, 0, st>>>(P); g_launches++; }
 	const uint64_t nb = (tiles + SCAN_BLOCK - 1) / SCAN_BLOCK;
 	if (tiles > 4 * SCAN_BLOCK && nb <= W.scan_cap) {
-		/* two million tile counts at 64 GiB: one block would take 1.6 ms over them */
+		/* a million tile counts at 32 GiB: too many for one block to walk, so a two-level scan */
 		k_scan_partial<<<(unsigned)nb, 1024, 0, st>>>(W.tile_counts, tiles, W.scan_sums, nullptr);
 		k_scan_tiles<<<1, 1024, 0, st>>>(W.scan_sums, W.scan_offs, nb, W.totals + 13);
 		k_scan_apply<<<(unsigned)nb, 1024, 0, st>>>(W.tile_counts, tiles, W.scan_offs, W.tile_offsets, nullptr);

@@ -1,4 +1,4 @@
-/* agrep_b200/csrc/dropin.c -- the drop-in layer: the reference's own entry points over the B200 engine.
+/* agrep_b200/csrc/dropin.c -- the drop-in layer: the reference's own entry points over the H100 engine.
  *
  * Exports, with the reference's exact (K&R) signatures:
  *     bitap()    bitap.c:78      asearch()  asearch.c:32     asearch0() asearch.c:574

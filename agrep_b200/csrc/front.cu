@@ -76,8 +76,8 @@ __device__ __forceinline__ void front_chunks(const FrontParams &P, const uint8_t
 	for (int c = 0; c < FRONT_CH; c++) {
 		const uint32_t idx = c * FRONT_THREADS + tid;
 		uint4 v = *reinterpret_cast<const uint4 *>(st + idx * 16);
-		/* the first word of the next chunk (a 4-way bank conflict, measured cheaper than SHFL + a predicated LDS:
-		 * 4905 vs 4787 GB/s, profiles/round1_front_variants.md) */
+		/* the first word of the next chunk (a 4-way bank conflict; the alternative is a SHFL + a predicated LDS for
+		 * the warp's last lane, which costs more issue slots) */
 		uint32_t x4 = *reinterpret_cast<const uint32_t *>(st + idx * 16 + 16);
 		if (COUNT) {
 			/* -n: the delimiter bytes of this chunk (SWAR: 0x80 where a byte equals the delimiter), summed over the warp =

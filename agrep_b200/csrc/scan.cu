@@ -30,7 +30,7 @@ thread_local char g_err[512];
 std::atomic<uint64_t> g_launches{0};
 
 extern "C" const char *agb_last_error(void) { return g_err; }
-extern "C" const char *agb_version(void) { return "agrep-b200 0.1 (sm_100a)"; }
+extern "C" const char *agb_version(void) { return "agrep-b200 0.1 (sm_90a)"; }
 extern "C" uint64_t agb_kernel_launches(void) { return g_launches.load(); }
 /* frees the per-device scratch of this process (bitmaps, candidate lists, pinned rings, streams, events); the next
  * scan allocates again */
@@ -186,8 +186,8 @@ static int records_launch(const agb_desc &d, Workspace &W, const void *d_text, u
 		CUDA_TRY(cudaMemcpyAsync(W.h_totals + 12, W.totals + 12, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
 		CUDA_TRY(cudaStreamSynchronize(st));
 		const unsigned long long ncand = W.h_totals[12];
-		/* list form while the survivors are sparse (20 B of scratch each; measured cross-over against the dense tile
-		 * kernel at about 5 % of the chunks: 'the' flags 11 % and runs 13.5 ms per 4 GiB as a list, 'government' 1.1 % and 1.7 ms) */
+		/* list form while the survivors are sparse (20 B of scratch each): one thread per candidate against the dense
+		 * tile kernel's walk over every byte; the cross-over is put at 5 % of the chunks ('the' flags 11 %, 'government' 1.1 %) */
 		const bool sparse = ncand <= n_chunks / 20 + 1024;
 		if (!sparse) {
 			CUDA_TRY(cudaMemsetAsync(W.totals + 1, 0, sizeof(unsigned long long), st));
@@ -316,10 +316,10 @@ static int adaptive_plan(const agb_desc &d, Workspace &W, const void *d_text, ui
 	for (int i = 0; i < ng; i++) g[i].cost = (double)W.h_gram[256 + i] / (double)threads;
 	/* dynamic program over the pattern positions: f[p][j][t] = least total rate of j disjoint grams inside [0, p), t of them
 	 * three bytes long */
-	/* what a three-byte group costs, in units of flag rate: measured on the benchmark pattern (beca|se e|ach flags 2.4 %
-	 * of the chunks instead of 4.5 %), stage 1 ran 22 % longer (14.5 instead of 11.8 ms per 64 GiB: the second polynomial
-	 * and one VIMNMX3 per window instead of half of one) and stage 1.5 did not get cheaper in proportion -- a mixed plan
-	 * only pays when the four-byte grams of a piece are really common */
+	/* what a three-byte group costs, in units of flag rate: on the benchmark pattern (beca|se e|ach flags 2.4 % of the
+	 * chunks instead of 4.5 %) stage 1 pays for a second polynomial and one VIMNMX3 per window instead of half of one,
+	 * and stage 1.5 does not get cheaper in proportion -- a mixed plan only pays when the four-byte grams of a piece
+	 * are really common */
 	const char *mp = getenv("AGB_PLAN_MIXED");           /* (tests force mixed plans with AGB_PLAN_MIXED=0) */
 	const double INF = 1e30, MIXED = mp ? atof(mp) : 0.03;
 	static double f[66][10][3]; static int from[66][10][3];   /* gram taken to get here, -1: position skipped */

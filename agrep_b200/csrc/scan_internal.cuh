@@ -32,7 +32,9 @@ extern std::atomic<uint64_t> g_launches;
 #define FRONT_STAGE_CHUNKS (FRONT_THREADS * FRONT_CH)     /* 1024 chunks = 16 KiB = 32 bitmap words per stage */
 #define FRONT_STAGE_BYTES  (FRONT_STAGE_CHUNKS * 16)
 #define FRONT_SLOT_BYTES   (FRONT_STAGE_BYTES + 16)       /* + the 16 bytes that follow: the last chunk's windows look 3 bytes ahead */
-#define FRONT_NST     2                                   /* stages in flight per CTA (32 KiB); 6 CTAs = 48 warps per SM: measured best */
+#define FRONT_NST     2                                   /* stages in flight per CTA (32 KiB); 6 CTAs = 48 warps per SM */
+/* tools/front_bench.cu on an H100 (16 GiB, 400 W power limit): this shape within the run-to-run spread (about 5 %) of the
+ * best ring shapes tried, 4 stages x 3 CTAs and 3 x 4 -- stage 1 is DRAM-bound there, so the ring shape matters little */
 #define FRONT_CTAS_PER_SM 6
 #define FRONT_WORDS_PER_STAGE (FRONT_STAGE_CHUNKS / 32)
 

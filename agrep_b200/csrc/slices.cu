@@ -149,9 +149,9 @@ k_records_slices(const RecParams P)
 		if (easy && !P.levels && !C.and_mode) {
 			/* Plain counting away from both ends of the text: every record counts (agrep.c:3811 only bites at the ends).
 			 * No branch on a close: one would be taken by one or two lanes in almost every other step of a warp (a line
-			 * ends every ~60 bytes) and the divergence costs far more than it skips (measured: 260 cycles per step and
-			 * warp).  The loop only resets the rows with selects and shifts two flags per step into a pair of 32-bit
-			 * histories -- "a record closed here", "and an end bit was up" (bitap.c:182 without -v; `;` patterns take
+			 * ends every ~60 bytes) and the divergence costs far more than it skips.  The loop only resets the rows with
+			 * selects and shifts two flags per step into a pair of 32-bit histories -- "a record closed here", "and an
+			 * end bit was up" (bitap.c:182 without -v; `;` patterns take
 			 * the general loop) -- which are counted and located with popc/clz/ffs once per 32 bytes. */
 			int first_j = -1, last_j = -1; bool first_found = false;
 			const bool inv = C.inverse != 0;

@@ -1,21 +1,23 @@
 #!/usr/bin/env python3
-"""bench.py -- the driver's measurement contract for agrep-b200.
+"""bench.py -- the throughput benchmark of agrep-b200 on H100.
 
 One "step" = one pass of the scan path over the whole synthetic corpus:
-    agrep -2 'because each' <64 GiB newline-delimited text>      (BASELINE.json configs[1])
+    agrep -2 'because each' <32 GiB newline-delimited text>      (BASELINE.json configs[1])
 i.e. stage 1 (k_front, the HBM-bound kernel) + stage 2 (k_records) + the ordered list of matching records;
-with N > 1 the 64 GiB are sharded by byte range over the ranks -- cut inside records, at multiples of 512 bytes -- and
+with N > 1 the 32 GiB are sharded by byte range over the ranks -- cut inside records, at multiples of 512 bytes -- and
 every rank calls agb_scan_sharded(): the cut rule runs on the device, the match lists are gathered with NCCL inside the
 library (C ABI, include/agrep_b200.h).
 
   python bench.py --gpus N --steps K --warmup W            our arm (one rank per GPU under torchrun)
   python bench.py --impl reference ...                      the reference's own CPU scan on the host cores
+  --dump-outputs DIR                                        also write what the last timed step returned (DIR/*.npy)
 
 Prints ONE JSON line (rank 0).  `value` = corpus bytes / device time (inputs resident in HBM);
 `e2e` = the same scan through agb_scan_host() on pinned HOST buffers, H2D and result D2H inside the timing;
-`roofline` = k_front's algorithmic bytes / its CUDA-event duration against MEASURED_PEAKS.json;
-`cpu_baseline` = the unmodified reference binary (oracle/_ref/agrep, built from /root/reference) on a
-bounded sample of the same corpus on the box's host cores.
+`roofline` = k_front's algorithmic bytes / its CUDA-event duration against MEASURED_PEAKS.json (else the H100 SXM
+data sheet's 3.35 TB/s);
+`cpu_baseline` = the unmodified reference binary (oracle/_ref/agrep, when oracle/Makefile could build it) on a
+bounded sample of the same corpus on the machine's host cores.
 """
 import argparse, ctypes, json, os, shutil, statistics, subprocess, sys, tempfile, threading, time
 
@@ -24,7 +26,7 @@ sys.path.insert(0, ROOT)
 
 PATTERN = "because each"          # 12-char literal made of two adjacent vocabulary words (SURVEY 8d)
 K = 2
-TOTAL_GIB = float(os.environ.get("AGB_BENCH_GIB", "64"))
+TOTAL_GIB = float(os.environ.get("AGB_BENCH_GIB", "32"))      # far beyond L2, with headroom on an 80 GB H100 shared with other work
 E2E_GIB = float(os.environ.get("AGB_BENCH_E2E_GIB", "4"))
 CPU_SAMPLE_MIB = int(os.environ.get("AGB_BENCH_CPU_MIB", "1024"))
 NEEDLE_EVERY = 4096               # one planted line per 16 MiB, with 0..3 substitutions
@@ -37,7 +39,7 @@ def peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(p["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (of measured)"
     except Exception:
-        return 6650.0, "fallback 6.65 TB/s (of fallback)"
+        return 3350.0, "H100 SXM data sheet 3.35 TB/s (not measured)"
 
 
 def host_cores():
@@ -93,7 +95,7 @@ def all_core_reference(ag, cores, shard_mib, steps=2):
 
 
 class ClockSampler:
-    """SM clock and throttle reasons DURING the timed region (B200_PROFILING.md's clocks line): NVML polled every 2 ms from a
+    """SM clock and throttle reasons DURING the timed region: NVML polled every 2 ms from a
     thread of this process (the timed region of a sharded run is a few tens of milliseconds, shorter than `nvidia-smi`
     takes to start), `nvidia-smi -lms` as the fallback; only the samples between begin() and end() count."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -259,7 +261,7 @@ def workload_config(n_gpus):
             "pattern": PATTERN, "k": K, "records": "newline", "corpus_gib": TOTAL_GIB,
             "parallelism": "1 GPU" if n_gpus == 1 else ("%d byte-range shards cut inside records (512-byte multiples), cut rule on the device, "
                                                            "ncclAllGather of 256-byte headers + match lists inside libagrepb200.so (agb_scan_sharded)" % n_gpus),
-            "l2": "input per GPU is far larger than the 126 MB L2; no flush needed",
+            "l2": "input per GPU is far larger than the 50 MB L2; no flush needed",
             "output": "count + ordered (begin,end) list of matching records"}
 
 
@@ -391,12 +393,32 @@ def secondary_workloads(ag, torch, corpus, n_local, stream, peak):
     return out
 
 
+DUMP_RECORD_ROWS = 2 << 20        # 32 MiB of (begin, end) + 16 MiB of row indices in float64: a sampled dump stays under 64 MB
+
+
+def dump_outputs(out_dir, res, recs):
+    """What the caller of the timed path receives from its last step: the match count and the ordered list of matching
+    records (begin, end byte offsets; exact in float64 below 2^53).  A list longer than DUMP_RECORD_ROWS is cut to a
+    sample of rows chosen with a fixed seed; records_index.npy says which."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    n = int(res.n_records)
+    np.save(os.path.join(out_dir, "counts.npy"), np.array([int(res.n_matched), n], dtype=np.float64))
+    rows = recs[:n, :2].cpu().numpy()
+    if n > DUMP_RECORD_ROWS:
+        idx = np.sort(np.random.default_rng(0).choice(n, DUMP_RECORD_ROWS, replace=False))
+        rows = rows[idx]
+        np.save(os.path.join(out_dir, "records_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "records.npy"), rows.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step returned as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else max(args.warmup, 1)
     if args.impl == "reference":
@@ -501,6 +523,8 @@ def main():
     launches = L.agb_kernel_launches() - launches0
     clocks = sampler.stop() if rank == 0 else None
     matched_total = gathered
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res, recs)
 
     # ---- end to end through the host-buffer entry point (pinned host memory, H2D + result D2H inside the timing)
     n_e2e = min(int(E2E_GIB * (1 << 30)), n_local - HR) // PAGE * PAGE
@@ -584,22 +608,10 @@ def main():
         peak, peak_src = peaks()
         fm = statistics.mean(front_ms)
         achieved = n_local / (fm * 1e-3) / 1e9
-        traffic = None
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "k_front_traffic.json")))
-        except Exception:
-            pass
         value = total / (ms_step * 1e-3) / 1e9
-        step_traffic = None
-        try:
-            step_traffic = json.load(open(os.path.join(ROOT, "profiles", "step_traffic.json")))
-        except Exception:
-            pass
         roofline_step = {"bound": "hbm", "what": "the whole step (stage 1 + stage 1.5 + record stage + ordered list), per GPU",
                          "achieved": n_local / (ms_step * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
-                         "frac": n_local / (ms_step * 1e-3) / 1e9 / peak, "algorithmic_bytes_per_step": n_local,
-                         "traffic": (step_traffic or {}).get("dram_bytes_per_step"),
-                         "traffic_note": (step_traffic or {}).get("note", "no ncu capture of a whole step yet")}
+                         "frac": n_local / (ms_step * 1e-3) / 1e9 / peak, "algorithmic_bytes_per_step": n_local}
         out = {
             "metric": "text_scan_throughput", "value": value, "unit": "GB/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True, "scaling": "strong",
@@ -608,9 +620,7 @@ def main():
             "roofline": {"bound": "hbm", "kernel": "k_front (stage 1, anchor filter)", "achieved": achieved, "peak": peak,
                          "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": n_local, "ms_per_launch": fm,
-                         "stage2_ms_per_step": statistics.mean(rec_ms),
-                         "traffic": (traffic or {}).get("dram_bytes_per_launch") if traffic else None,
-                         "traffic_note": (traffic or {}).get("note") if traffic else "no ncu --set full capture yet"},
+                         "stage2_ms_per_step": statistics.mean(rec_ms)},
             "roofline_step": roofline_step,
             "e2e": {"value": e2e_val, "unit": "GB/s", "h2d_bytes_per_step": n_e2e, "d2h_bytes_per_step": 128 + 32 * int(nrec),
                     "what": "agb_scan_host() on a pinned host buffer holding the first %.1f GiB of each rank's shard; "

@@ -1,4 +1,4 @@
-/* include/agrep_b200.h -- C ABI of libagrepb200.so: the B200 scan engine behind agrep's scan path.
+/* include/agrep_b200.h -- C ABI of libagrepb200.so: the H100 scan engine behind agrep's scan path.
  *
  * Plain C, pointers and sizes only.  Two layers:
  *
@@ -12,7 +12,7 @@
  *      asearch0(), asearch1(), sgrep(), fill_buf(), alloc_buf(), free_buf() with the reference's own
  *      signatures, reading the reference's globals, so the reference's exec() links against it unchanged.
  *
- * There is no CPU fallback: every agb_scan_* call runs the sm_100a kernels and fails with
+ * There is no CPU fallback: every agb_scan_* call runs the sm_90a kernels and fails with
  * AGB_ERR_CUDA when no device is usable.
  */
 #ifndef AGREP_B200_H

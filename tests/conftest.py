@@ -1,4 +1,4 @@
-import os, sys, subprocess, pytest
+import os, sys, subprocess
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -6,14 +6,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
-    # build the checker (oracle) and, when /root/reference is present, oracle/_ref
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
+    # build the checker (oracle) and, when the reference sources are present, oracle/_ref
     subprocess.run(["make", "-s", "-C", os.path.join(ROOT, "oracle"), "all"], check=True,
                    stdout=subprocess.DEVNULL)
-
-
-@pytest.fixture(scope="session")
-def ref_agrep():
-    """Path of the unmodified reference binary built by oracle/Makefile (None if never built)."""
-    p = os.path.join(ROOT, "oracle", "_ref", "agrep")
-    return p if os.path.exists(p) else None

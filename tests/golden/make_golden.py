@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Generates tests/golden/*.json from the UNMODIFIED reference (oracle/_ref, built by oracle/Makefile
-from /root/reference).  Run in the build container only:  python tests/golden/make_golden.py
+"""Generates tests/golden/* from the UNMODIFIED reference (oracle/_ref, built by oracle/Makefile from the reference
+sources).  Run where oracle/_ref exists:  python tests/golden/make_golden.py
 Inputs are the seeded corpora of tests/_corpus.py, so only the answers are committed."""
 import json, os, re, subprocess, sys, tempfile
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -108,6 +108,23 @@ def main():
     CP = ((E * 257) * 3).in_dll(lib, "CP")
     json.dump([CP[2][i].l1 if CP[2][i].m == 0 else i for i in range(256)], open(os.path.join(HERE, "lut_lower1.json"), "w"))
     print("wrote", len(out["scan"]), "scan cases,", len(out["dump"]), "dumps")
+    # the stand-alone command line's cases (tests/test_gpu_dropin.py): exit status and stdout digest, run in the files'
+    # directory so that the file names printed do not depend on where it ran
+    import hashlib
+    import test_gpu_dropin as tg
+    cli = {}
+    with tempfile.TemporaryDirectory() as d:
+        tg.make_files(d)
+        for args, names in tg.CLI_CASES:
+            p = subprocess.run([REF + "/agrep"] + args + names, capture_output=True, timeout=300, stdin=subprocess.DEVNULL, cwd=d)
+            cli[" ".join(args + names)] = {"rc": p.returncode, "bytes": len(p.stdout), "sha256": hashlib.sha256(p.stdout).hexdigest()}
+    json.dump(cli, open(os.path.join(HERE, "cli_stdout.json"), "w"), indent=1, sort_keys=True)
+    # tests/test_oracle_vs_reference.py asks the reference binary itself and stores its answers (reference_answers.json.gz):
+    # every test of the module must have run and passed before the new answers replace the committed ones
+    answers = os.path.join(HERE, "reference_answers.json.gz")
+    subprocess.run([sys.executable, "-m", "pytest", "-q", "-p", "no:cacheprovider", os.path.join(os.path.dirname(HERE), "test_oracle_vs_reference.py")],
+                   env=dict(os.environ, AGB_RECORD_REFERENCE=REF + "/agrep"), check=True)
+    os.replace(answers + ".new", answers)
 
 
 if __name__ == "__main__":

@@ -1,8 +1,10 @@
 """The drop-in proof: the reference program linked against libagrepb200_dropin.so (oracle/_ref/agrep_dropin:
 the reference's own main(), option parser, exec() and output(); only bitap/asearch/asearch0/asearch1/sgrep/
 fill_buf come from this repo and run on the GPU) must print byte-for-byte what the unmodified reference
-(oracle/_ref/agrep) prints.  Both binaries are built here by oracle/Makefile and travel to the GPU box."""
-import os, subprocess, tempfile
+(oracle/_ref/agrep) prints.  Both binaries are built by oracle/Makefile where the reference sources are at hand; the
+tests that run them skip elsewhere.  The stand-alone command line is checked against the reference's output stored in
+tests/golden/cli_stdout.json."""
+import hashlib, json, os, subprocess
 import pytest
 import _corpus
 
@@ -14,11 +16,8 @@ DROP = os.path.join(ROOT, "oracle", "_ref", "agrep_dropin")
 from _corpus import overlap_text
 
 
-@pytest.fixture(scope="module")
-def files():
-    if not (os.path.exists(REF) and os.path.exists(DROP)):
-        pytest.skip("oracle/_ref binaries not built")
-    d = tempfile.mkdtemp(prefix="agb_dropin_")
+def make_files(d):
+    """the seeded input files of CASES, written into directory d; returns {name: path}"""
     paths = {}
     for name, data in (("a.txt", _corpus.make_text(3000, seed=11)), ("b.txt", _corpus.make_text(2000, seed=12, trailing_newline=False)),
                        ("para.txt", _corpus.make_text(2500, seed=13, paragraphs=True)),
@@ -29,14 +28,21 @@ def files():
 
         paths[name] = os.path.join(d, name)
         open(paths[name], "wb").write(data)
-    yield paths
-    for p in paths.values():
-        os.unlink(p)
-    os.rmdir(d)
+    return paths
 
 
-def run(binary, args):
-    p = subprocess.run([binary] + args, capture_output=True, timeout=120, stdin=subprocess.DEVNULL)
+@pytest.fixture(scope="module")
+def files(tmp_path_factory):
+    return make_files(str(tmp_path_factory.mktemp("agb_dropin_")))
+
+
+def needs_reference():
+    if not (os.path.exists(REF) and os.path.exists(DROP)):
+        pytest.skip("oracle/_ref binaries not built")
+
+
+def run(binary, args, cwd=None):
+    p = subprocess.run([binary] + args, capture_output=True, timeout=120, stdin=subprocess.DEVNULL, cwd=cwd)
     return p.returncode, p.stdout, p.stderr
 
 
@@ -79,6 +85,7 @@ CASES = [
 
 @pytest.mark.parametrize("args,names", CASES)
 def test_same_stdout_as_reference(files, args, names):
+    needs_reference()
     fl = [files[n] for n in names]
     r = run(REF, ["-V0"] + args + fl)
     d = run(DROP, ["-V0"] + args + fl)
@@ -88,20 +95,22 @@ def test_same_stdout_as_reference(files, args, names):
 
 
 CLI = os.path.join(ROOT, "agrep_b200", "agrep-b200")
+CLI_GOLDEN = os.path.join(ROOT, "tests", "golden", "cli_stdout.json")
 CLI_CASES = [c for c in CASES if not any(a in ("-L2", "-s") or a.startswith("-S") for a in c[0]) and c[0][-1] not in ("a#d;world",)
              and "semi.txt" not in c[1]]
 
 
 @pytest.mark.parametrize("args,names", CLI_CASES)
 def test_standalone_cli_prints_what_the_reference_prints(files, args, names):
-    """agrep-b200 (agrep_b200/csrc/agrep_main.c): our own main() + output() restatement over the engine."""
+    """agrep-b200 (agrep_b200/csrc/agrep_main.c): our own main() + output() restatement over the engine, against the
+    exit status and stdout (length and SHA-256) the unmodified reference gave for the same command in the files'
+    directory -- default verbosity: with the "Grand Total" line."""
     if not os.path.exists(CLI):
         pytest.skip("agrep-b200 not built")
-    fl = [files[n] for n in names]
-    r = run(REF, args + fl)                      # default verbosity: with the "Grand Total" line
-    d = run(CLI, args + fl)
-    assert d[1] == r[1]
-    assert d[0] == r[0]
+    want = json.load(open(CLI_GOLDEN))[" ".join(args + names)]
+    rc, out, _ = run(CLI, args + names, cwd=os.path.dirname(files[names[0]]))
+    assert (len(out), hashlib.sha256(out).hexdigest()) == (want["bytes"], want["sha256"]), out[:300]
+    assert rc == want["rc"]
 
 
 MEM = os.path.join(ROOT, "oracle", "_ref", "memagrep_cli")
@@ -115,6 +124,7 @@ def test_memory_mode_through_the_dropin(files, args, name):
     """memagrep() (agrep.c:3282; scan loop bitap.c:309-446): the reference's in-memory entry point with the scan objects
     replaced by the drop-in layer (fd == -1: the caller's buffer is scanned, no delimiter is appended behind it, so an
     undelimited last record is not reported -- by -c either) prints and returns what the unmodified one does."""
+    needs_reference()
     if not (os.path.exists(MEM) and os.path.exists(MEMDROP)):
         pytest.skip("oracle/_ref memagrep drivers not built")
     r = run(MEM, [files[name], "-V0"] + args)

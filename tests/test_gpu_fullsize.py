@@ -1,19 +1,19 @@
-"""Parity at BASELINE.json's full size (64 GiB on one B200) through size-independent properties -- the oracle
-cannot scan 64 GiB in seconds, so we use what the domain offers:
+"""Parity at BASELINE.json's full size (32 GiB on one H100) through size-independent properties -- the oracle
+cannot scan 32 GiB in seconds, so we use what the domain offers:
   * additivity: the corpus is made of independent pages, so count(whole) == sum of count(shard) for any
     page-aligned sharding (a checksum of checksums), and the whole-corpus record list is the concatenation;
   * sampling: on 64 randomly chosen 1 MiB windows the device scan equals the oracle bit for bit (the window is
     regenerated on the host by the same generator);
   * monotonicity in k (the rows are nested, asearch.c:98-114) and determinism (two runs, identical lists);
   * completeness on planted needles: every planted line with e <= k substitutions is reported.
-Size: AGB_FULLSIZE_GIB (default 64; the test skips if the device cannot hold it)."""
+Size: AGB_FULLSIZE_GIB (default 32; the test skips if the device cannot hold it)."""
 import os, random
 import pytest
 import _oracle
 import agrep_b200 as ag
 
 pytestmark = pytest.mark.gpu
-GIB = float(os.environ.get("AGB_FULLSIZE_GIB", "64"))
+GIB = float(os.environ.get("AGB_FULLSIZE_GIB", "32"))
 PAGE = 4096
 NEEDLE, EVERY, MAXE = "because each", 4096, 3
 

@@ -25,7 +25,7 @@ def test_library_exports_declared_symbols():
     for name in sorted(declared):
         assert hasattr(L, name), name
     assert set(_lib.EXPORTS) <= declared
-    assert b"sm_100a" in L.agb_version()
+    assert b"sm_90a" in L.agb_version()
 
 
 @pytest.mark.parametrize("name", sorted(G["dump"]))

@@ -1,6 +1,6 @@
 // tools/front_bench.cu -- development microbenchmark (not product): inner-compare variants of the stage-1
 // anchor kernel on synthetic text, to pick the instruction mix with measurements instead of guesses.
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o tools/front_bench tools/front_bench.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o tools/front_bench tools/front_bench.cu
 // run:   tools/front_bench [GiB]
 #include <cuda_runtime.h>
 #include <cstdio>
@@ -214,9 +214,9 @@ int main(int argc, char **argv)
 	double gib = argc > 1 ? atof(argv[1]) : 4.0;
 	uint64_t bytes = (uint64_t)(gib * (1ull << 30)) & ~511ull;
 	uint32_t *text, *bitmap; CK(cudaMalloc(&text, bytes + 64)); CK(cudaMalloc(&bitmap, bytes / 128 + 64));
-	fill<<<148 * 8, 256>>>(text, bytes / 4, 1); CK(cudaDeviceSynchronize());
 	cudaDeviceProp pr; CK(cudaGetDeviceProperties(&pr, 0));
 	int sms = pr.multiProcessorCount;
+	fill<<<sms * 8, 256>>>(text, bytes / 4, 1); CK(cudaDeviceSynchronize());
 	printf("device %s, %d SMs, %.2f GiB text\n", pr.name, sms, gib);
 	P p; p.text = (const uint4 *)text; p.bitmap = bitmap; p.n_chunks = bytes / 16; p.n_words = p.n_chunks / 32;
 	const char *a[8] = { "beca", "use ", "each", "gove", "rnme", "ntal", "xyzw", "qqqq" };

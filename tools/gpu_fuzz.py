@@ -1,4 +1,4 @@
-"""tools/gpu_fuzz.py [seed] -- development fuzz on a B200: random metacharacter patterns and options, the GPU path
+"""tools/gpu_fuzz.py [seed] -- development fuzz on an H100: random metacharacter patterns and options, the GPU path
 (agb_scan_host, list + ordinals, and count only) against the oracle.  Found the -p + multi-byte delimiter case.
 The committed, shorter version is tests/test_gpu_parity.py::test_random_metachar_differential."""
 import random, sys, os
