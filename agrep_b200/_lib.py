@@ -9,14 +9,16 @@ LIB_PATH = os.path.join(HERE, "libagrepb200.so")
 AGB_MAXERR, AGB_MAXDELIM, AGB_MAXANCHOR = 8, 8, 24
 WANT_COUNT, WANT_RECORDS, WANT_ORDINALS, WANT_LEVELS = 0, 1, 2, 4
 PLAN_ALL, PLAN_ANCHORS = 0, 1
-ENGINE_NAMES = {0: "bitap", 1: "asearch", 2: "asearch0", 3: "asearch1", 4: "sgrep_bm"}
+ENGINE_NAMES = {0: "bitap", 1: "asearch", 2: "asearch0", 3: "asearch1", 4: "sgrep_bm", 5: "regex"}
+ENGINE_REGEX = 5
+REGEX_MAXPOS = 63
 
 
 class Options(C.Structure):
     _fields_ = [("k", C.c_int32), ("nocase", C.c_int32), ("wordbound", C.c_int32), ("wholeline", C.c_int32),
                 ("inverse", C.c_int32), ("linenum", C.c_int32), ("ins_free", C.c_int32),
                 ("cost_i", C.c_int32), ("cost_s", C.c_int32), ("cost_d", C.c_int32),
-                ("bestmatch", C.c_int32), ("reserved", C.c_int32), ("delim", C.c_char_p)]
+                ("bestmatch", C.c_int32), ("regex", C.c_int32), ("delim", C.c_char_p)]
 
 
 class Desc(C.Structure):
@@ -37,6 +39,10 @@ class Desc(C.Structure):
                 ("delim_fold", C.c_uint8 * (2 * AGB_MAXDELIM + 2)), ("pad_", C.c_uint8 * 2)]
 
 
+class Regex(C.Structure):
+    _fields_ = [("follow", C.c_uint64 * (REGEX_MAXPOS + 1)), ("head", C.c_int32), ("tail", C.c_int32), ("pad", C.c_int32 * 2)]
+
+
 class Record(C.Structure):
     _fields_ = [("begin", C.c_int64), ("end", C.c_int64), ("ordinal", C.c_int64), ("level", C.c_int32), ("pad", C.c_int32)]
 
@@ -54,6 +60,7 @@ class CorpusSpec(C.Structure):
 
 
 EXPORTS = ["agb_fill_ordinals", "agb_compile", "agb_pattern_free", "agb_pattern_desc", "agb_pattern_from_desc", "agb_scan_device",
+           "agb_pattern_regex", "agb_pattern_from_regex",
            "agb_scan_host", "agb_scan_fd", "agb_bestmatch_device", "agb_corpus_fill_device", "agb_corpus_fill_host",
            "agb_last_error", "agb_device_count", "agb_set_device", "agb_version", "agb_kernel_launches", "agb_shutdown",
            "agb_text_from_host", "agb_text_from_fd", "agb_text_free", "agb_text_size", "agb_text_device", "agb_scan_text",
@@ -86,6 +93,9 @@ def lib():
     L.agb_pattern_desc.argtypes = [C.c_void_p]
     L.agb_pattern_desc.restype = C.POINTER(Desc)
     L.agb_pattern_from_desc.argtypes = [C.POINTER(Desc), C.POINTER(C.c_void_p), C.c_char_p, C.c_size_t]
+    L.agb_pattern_regex.argtypes = [C.c_void_p]
+    L.agb_pattern_regex.restype = C.POINTER(Regex)
+    L.agb_pattern_from_regex.argtypes = [C.POINTER(Desc), C.POINTER(Regex), C.POINTER(C.c_void_p), C.c_char_p, C.c_size_t]
     L.agb_scan_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(Result)]
     L.agb_scan_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_uint64, C.POINTER(Result)]
     L.agb_scan_fd.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint64, C.POINTER(Result)]

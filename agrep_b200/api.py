@@ -6,8 +6,8 @@ switches by name; `scan_*` return what exec() derives from the scan functions: n
 (lasti, print_end, j) triples handed to output() (agrep.c:3805).  All work happens in libagrepb200.so."""
 import ctypes as C
 from . import _lib
-from ._lib import (Options, Desc, Record, Result, CorpusSpec, WANT_COUNT, WANT_RECORDS, WANT_ORDINALS, WANT_LEVELS,
-                   PLAN_ALL, PLAN_ANCHORS, ENGINE_NAMES)
+from ._lib import (Options, Desc, Regex, Record, Result, CorpusSpec, WANT_COUNT, WANT_RECORDS, WANT_ORDINALS, WANT_LEVELS,
+                   PLAN_ALL, PLAN_ANCHORS, ENGINE_NAMES, ENGINE_REGEX)
 
 
 class AgrepError(Exception):
@@ -15,10 +15,12 @@ class AgrepError(Exception):
 
 
 class Pattern:
-    """agb_compile(): checksg() + preprocess() + maskgen() of the reference, plus the device plan."""
+    """agb_compile(): checksg() + preprocess() + maskgen() of the reference, plus the device plan.
+    regex: accept regular expressions (a pattern with an unescaped '|' or '*': re() of the reference, k <= 4, lines);
+    without it such a pattern is refused."""
 
     def __init__(self, pattern, k=0, nocase=False, wordbound=False, wholeline=False, inverse=False,
-                 linenum=False, ins_free=False, cost_i=0, cost_s=0, cost_d=0, bestmatch=False, delim=None):
+                 linenum=False, ins_free=False, cost_i=0, cost_s=0, cost_d=0, bestmatch=False, delim=None, regex=False):
         if isinstance(pattern, str):
             pattern = pattern.encode("latin-1")
         if isinstance(delim, str):
@@ -26,7 +28,7 @@ class Pattern:
         self.pattern = pattern
         self.opts = Options(k=k, nocase=int(nocase), wordbound=int(wordbound), wholeline=int(wholeline),
                             inverse=int(inverse), linenum=int(linenum), ins_free=int(ins_free),
-                            cost_i=cost_i, cost_s=cost_s, cost_d=cost_d, bestmatch=int(bestmatch), delim=delim)
+                            cost_i=cost_i, cost_s=cost_s, cost_d=cost_d, bestmatch=int(bestmatch), regex=int(regex), delim=delim)
         self._h = C.c_void_p()
         err = C.create_string_buffer(512)
         rc = _lib.lib().agb_compile(pattern, C.byref(self.opts), C.byref(self._h), err, 512)
@@ -37,6 +39,12 @@ class Pattern:
     def desc(self):
         # a copy: the C object dies with this Pattern
         return Desc.from_buffer_copy(_lib.lib().agb_pattern_desc(self._h).contents)
+
+    @property
+    def regex(self):
+        """the follow sets of a regular expression (a copy), None for every other engine"""
+        r = _lib.lib().agb_pattern_regex(self._h)
+        return Regex.from_buffer_copy(r.contents) if r else None
 
     def __del__(self):
         try:

@@ -4,7 +4,8 @@
  * reference's exec()/output() print for them (agrep.c:3332-3752, 3805-3956): -# -c -i -w -x -v -n -p -I# -S# -D#
  * -d delim -B -y -l -h -s -b -t -V# -e pat, one or more files.  It is NOT the drop-in (that is the reference's
  * own main() linked against libagrepb200_dropin.so, INTEGRATION.md); it exists so the engine can be used
- * where the reference's sources are not around.  No regex, no -f/-m multi-pattern, no -r (out of scope, DESIGN.md 7).
+ * where the reference's sources are not around.  Regular expressions (an unescaped '|' or '*') run on the device as
+ * re() would (DESIGN.md 3.6).  No -f/-m multi-pattern, no -r (out of scope, DESIGN.md 7).
  */
 #include "agrep_b200.h"
 #include <stdio.h>
@@ -23,6 +24,16 @@ static void usage(void)
 {
 	fprintf(stderr, "usage: %s [-#cdehilnpstvwxyBDIS] [-d delim] [-e] pattern [files]\n", prog);
 	exit(2);
+}
+
+/* an unescaped '|' or '*' (preproce.c:139-142) */
+static int is_regex(const char *s)
+{
+	for (; *s; s++) {
+		if (*s == '\\') { if (!*++s) break; }
+		else if (*s == '|' || *s == '*') return 1;
+	}
+	return 0;
 }
 
 static unsigned char *slurp(const char *path, size_t *n, int L, const unsigned char *dpat)
@@ -50,6 +61,16 @@ static unsigned char *slurp(const char *path, size_t *n, int L, const unsigned c
 static void print_record(const unsigned char *hb, const agb_desc *d, const agb_record *rec, const char *fname)
 {
 	long long i1 = rec->begin + 1, i2 = rec->end, j = rec->ordinal; int L = d->L;   /* buffer indexes (lasti, print_end) */
+	if (d->engine == AGB_ENGINE_REGEX) {
+		/* re() prints through r_output(), agrep.c:1919-: the prefixes, then the line with its newline (no output() quirks) */
+		num_of_matched++;
+		if (COUNT || SILENT) return;
+		if (FNAME) printf("%s: ", fname);
+		if (LINENUM) printf("%lld: ", j - 1);
+		if (BYTECOUNT) printf("%lld= ", (long long)rec->end);
+		fwrite(hb + rec->begin + 2, 1, (size_t)(rec->end - rec->begin), stdout);       /* hb[x + 1] is byte x of the text */
+		return;
+	}
 	if (i1 > i2) return;                                                             /* agrep.c:3811 */
 	num_of_matched++;
 	if (COUNT || SILENT) return;
@@ -102,6 +123,7 @@ int main(int argc, char **argv)
 {
 	agb_options o; agb_pattern *p = NULL; char err[256]; const char *pattern = NULL; int ai, nfiles, rc;
 	memset(&o, 0, sizeof o);
+	o.regex = 1;
 	if (argc > 0 && argv[0]) { const char *s = strrchr(argv[0], '/'); prog = s ? s + 1 : argv[0]; }
 	for (ai = 1; ai < argc && argv[ai][0] == '-' && argv[ai][1]; ai++) {
 		const char *q = argv[ai] + 1; int stop = 0;
@@ -133,15 +155,26 @@ int main(int argc, char **argv)
 	if (COUNT && LINENUM) { LINENUM = 0; fprintf(stderr, "%s: -n option ignored with -c\n", prog); }   /* compat.c:30-33 (the engine choice stays) */
 	FNAME = nfiles > 1 && !NOFILENAME;
 	if (o.delim && strlen(o.delim) == 1 && (o.delim[0] == '\n' || o.delim[0] == '$' || o.delim[0] == '^')) OUTTAIL = 1;   /* agrep.c:2290 */
+	if (is_regex(pattern) && (o.cost_i || o.cost_s || o.cost_d)) {
+		fprintf(stderr, "%s: -D#, -I#, or -S# option is ignored for regular expression pattern\n", prog);   /* compat.c:75-79 */
+		o.cost_i = o.cost_s = o.cost_d = 0;
+	}
 	rc = agb_compile(pattern, &o, &p, err, sizeof err);
-	if (rc) { fprintf(stderr, "%s: %s\n", prog, err); return 255; }
+	if (rc) {
+		fprintf(stderr, "%s: %s\n", prog, err);
+		/* bitap.c:96-104 refuses k > 4 at scan time, after main() has set up its output: the total is still printed */
+		if (is_regex(pattern) && o.k > 4 && VERBOSE > 0 && o.k <= AGB_MAXERR) printf("Grand Total: 0 match(es) found.\n");
+		return 255;
+	}
 
 	scan_files(p, argv + ai, nfiles, 0);
 	if (BESTMATCH && num_of_matched == 0 && nfiles > 0) {
 		/* agrep.c:3582-3728: nothing matched -> counting passes at D = 1, 2, ... < M, <= 8 until something matches,
 		 * report, ask (unless -y), then one printing pass at that D */
-		const int M = agb_pattern_desc(p)->M; int k, best = -1;
+		const int M = agb_pattern_desc(p)->M, regex = agb_pattern_desc(p)->engine == AGB_ENGINE_REGEX; int k, best = -1;
 		for (k = 1; k < M && k <= AGB_MAXERR && best < 0; k++) {
+			/* a regular expression allows 4 errors at most: the reference's sweep goes on to k = 5 and fails there (SURVEY 8c) */
+			if (regex && k > 4) { fprintf(stderr, "%s: no match within 4 errors, the most a regular expression allows\n", prog); break; }
 			agb_pattern *pk; o.k = k;
 			if (agb_compile(pattern, &o, &pk, err, sizeof err)) break;
 			num_of_matched = 0;

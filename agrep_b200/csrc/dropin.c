@@ -11,7 +11,9 @@
  * What happens per call: the globals maskgen() left behind become an agb_desc; the text goes to HBM and through
  * the CUDA stages; the ordered record list that comes back is replayed through the reference's own output()
  * (agrep.c:3805), which keeps every formatting switch (-n -b -h -l -c -s ...) byte-identical.  Regular
- * expressions keep going to the reference's re()/re1() (agrep.c:468,1267), as bitap.c:96-111 does.
+ * expressions that the reference gives to re() (at most SHORTREG positions, bitap.c:105-106) run on the engine as
+ * well -- the descriptor and follow sets from Mask[], NO_ERR_MASK, HEAD/TAIL and table[][] -- and are replayed
+ * through the reference's r_output() (agrep.c:1919); longer ones keep going to the reference's re1() (agrep.c:468).
  *
  * How the text gets there (the fill_buf() loop of bitap.c:143,450-477 replaced):
  *   - a regular file is never slurped: it is read(2) straight into the engine's pinned ring and on to the device
@@ -50,7 +52,10 @@ extern unsigned char *agrep_inbuffer, *agrep_outbuffer;
 extern FILE *agrep_finalfp;
 extern int glimpse_clientdied;
 extern int output();           /* agrep.c:3805 */
-extern int re(), re1();        /* agrep.c:1267, 468 */
+extern int r_output();         /* agrep.c:1919 */
+extern int re1();              /* agrep.c:468 */
+extern int HEAD, TAIL;         /* preproce.c:231-236, 334-339 */
+extern int table[32][32];      /* follow sets of the regex positions, follow.c:210-255 (agrep.c:219, WORD = 32) */
 
 /* ---- fill_buf / alloc_buf / free_buf: same contracts (other reference files, e.g. newmgrep.c and file_out(),
  * keep calling them) ---- */
@@ -405,12 +410,81 @@ done:
 	return ret;
 }
 
+/* re() (agrep.c:1267-1917) on the engine.  The words are the reference's: Mask[] and NO_ERR_MASK as maskgen() left them
+ * (position p at bit M - p, as in agb_desc), Init[0] = Bit[base] | (HEAD ? Bit[base+1] : 0) (agrep.c:1285-1286), and the
+ * follow sets read from table[][] the way compute_next() reads them (agrep.c:405-415): positions 1 .. M-1, at most ten
+ * entries each -- the reference's cap is kept on purpose here, the goal being its own output (SURVEY 8c).  Each matching
+ * line goes through the reference's r_output() in a buffer of its own: '\n', the line, its newline. */
+static int regex_scan(int fd, int M, int D)
+{
+	agb_desc d; agb_regex rx; agb_pattern *p = NULL; agb_result res; agb_record *recs = NULL; source src;
+	unsigned char *buf = NULL; size_t bufcap = 0; unsigned long long i; int c, q, j, rc, ret = 0; char err[256];
+	const unsigned char nl = '\n';
+	memset(&d, 0, sizeof d); memset(&rx, 0, sizeof rx);
+	for (c = 0; c < 256; c++) d.mask[c] = Mask[c];
+	d.noerr = NO_ERR_MASK;
+	d.init0 = (1ull << M) | (HEAD ? 1ull << (M - 1) : 0);
+	d.init1 = d.init0 | 1;
+	d.endpos = 1; d.dmask = ~0ull;
+	d.M = M; d.L = 1; d.delim[0] = '\n'; d.k = D; d.engine = AGB_ENGINE_REGEX; d.inverse = INVERSE;
+	d.cost_i = d.cost_s = d.cost_d = 1;
+	rx.follow[0] = 1ull << (M - 1);                          /* compute_next's constant k >> 1: the start feed */
+	for (q = 1; q < M; q++)
+		for (j = 0; j < 10 && table[q][j] > 0; j++) rx.follow[q] |= 1ull << (M - table[q][j]);
+	rx.head = HEAD; rx.tail = TAIL;
+	rc = agb_pattern_from_regex(&d, &rx, &p, err, sizeof err);
+	if (rc) { fprintf(stderr, "%s: %s\n", Progname, err); errno = AGREP_ERROR; return -1; }
+	source_open(fd, &src);
+	if (src.kind < 0) { agb_pattern_free(p); fprintf(stderr, "%s: out of memory\n", Progname); errno = AGREP_ERROR; return -1; }
+	if (COUNT && !FILENAMEONLY && fd != -1) {               /* r_output() would only count (agrep.c:1926-1927) */
+		rc = source_scan(p, &src, AGB_WANT_COUNT, NULL, 0, &res);
+		if (rc) ret = fail("scan");
+		else num_of_matched += (int)res.n_matched;
+		goto done;
+	}
+	rc = scan_records(p, &src, AGB_WANT_ORDINALS, &recs, &res);
+	if (rc) { ret = fail("scan"); goto done; }
+	for (i = 0; i < res.n_records; i++) {
+		const agb_record *r = &recs[i];
+		if (fd == -1 && r->end >= (long long)src.n) continue;     /* memory mode appends no newline */
+		if (FILENAMEONLY && (NEW_FILE || !POST_FILTER)) {           /* agrep.c:1334-1356 */
+			num_of_matched++;
+			if (agrep_finalfp != NULL) fprintf(agrep_finalfp, "%s\n", CurrentFileName);
+			else {
+				size_t fl = strlen(CurrentFileName);
+				if (agrep_outpointer + (int)fl + 1 >= agrep_outlen) { ret = -1; break; }
+				memcpy(agrep_outbuffer + agrep_outpointer, CurrentFileName, fl);
+				agrep_outbuffer[agrep_outpointer + fl] = '\n';
+				agrep_outpointer += (int)fl + 1;
+			}
+			NEW_FILE = 0;
+			break;
+		}
+		{
+			/* record_bytes() gives [begin, end + 1): the opening newline (virtual for the first line), the line, its newline */
+			unsigned char *rb = record_bytes(&src, r, &nl, 1, &buf, &bufcap);
+			const int at = (int)(r->end - r->begin);            /* index of the closing newline */
+			if (!rb) { ret = -1; errno = AGREP_ERROR; break; }
+			rb[0] = '\n';
+			CurrentByteOffset = (int)r->end;                    /* where re() leaves it at the newline (agrep.c:1329-1331) */
+			if (-1 == r_output(rb, at, at + 1, (int)r->ordinal)) { ret = -1; break; }
+		}
+		if ((LIMITOUTPUT > 0 && LIMITOUTPUT <= num_of_matched) ||
+		    (LIMITPERFILE > 0 && LIMITPERFILE <= num_of_matched - prev_num_of_matched)) break;     /* agrep.c:1359-1363 */
+	}
+done:
+	free(recs); free(buf); source_close(&src); agb_pattern_free(p);
+	return ret;
+}
+
 int bitap(char old_D_pat[], char *Pattern, int fd, int M, int D)
 {
-	if (REGEX) {                                            /* bitap.c:96-111: stays with the reference's NFA code */
+	if (REGEX) {                                            /* bitap.c:96-111 */
 		if (D > 4) { fprintf(stderr, "%s: the maximum number of erorrs allowed for full regular expressions is 4\n", Progname); errno = AGREP_ERROR; return -1; }
 		D_length = (int)strlen(old_D_pat);
-		return M <= SHORTREG ? re(fd, M, D) : re1(fd, M, D);
+		/* re1() (16-30 positions) prints wrong line numbers and misses matches with errors (SURVEY 8c): the reference's
+		 * own output for those is its re1()'s, so it keeps running it */
+		return M <= SHORTREG ? regex_scan(fd, M, D) : re1(fd, M, D);
 	}
 	if (D > 0 && JUMP == 1) return scan_and_replay(old_D_pat, (const unsigned char *)Pattern, fd, M, D, AGB_ENGINE_ASEARCH1);   /* bitap.c:113-116 */
 	if (D > 4) return scan_and_replay(old_D_pat, (const unsigned char *)Pattern, fd, M, D, AGB_ENGINE_ASEARCH0);               /* asearch.c:50-52 */

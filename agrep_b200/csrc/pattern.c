@@ -118,6 +118,56 @@ static int add_sep(build_t *b, int is_and, int L, char *err, size_t errlen)
 	return 0;
 }
 
+/* one "[...]" class (maskgen.c:96-127); s[*i] is the '[', *i is left on the closing ']'.  regex: '.' inside the class
+ * also matches '\n' (maskgen.c:243), and a range that parse_cset() refuses (parse.c:81-120) is an error */
+static int add_class(build_t *b, const unsigned char *s, int *pi, int n, const agb_options *o, int regex, char *err, size_t errlen)
+{
+	pos_t *p = new_pos(b); int compl_ = 0, closed = 0, esc, i = *pi;
+	uint64_t keep[4];
+	if (!p) { if (regex) FAIL("regular expression too long"); FAIL("pattern too long (has > %d chars)", WIDTH); }
+	if (b->no_error) p->prot = 1;
+	i++;
+	if (i < n && s[i] == '^') { compl_ = 1; i++; }
+	{   /* maskgen.c:104-116 keeps the class as (low, high) pairs: a symbol opens the pair (c, c), "-x" replaces the high
+	     * end of the last pair -- so a descending range like z-a matches nothing, not even z */
+		int plo[2 * WIDTH], phi[2 * WIDTH], np = 0, q;
+		for (; i < n; i++) {
+			int cc = map_sym(s, &i, n, 1, &esc);
+			if (!esc && cc == S_RRANGE) { closed = 1; break; }
+			if (!esc && cc == S_HYPHEN) {                              /* class[k-1] = next symbol */
+				int hi;
+				if (regex && np == 0) FAIL("illegal regular expression");
+				i++;
+				if (i >= n) break;
+				hi = map_sym(s, &i, n, 1, &esc);
+				if (o->nocase && is_upper(hi)) hi += 32;
+				if (regex && np > 0 && hi < plo[np - 1]) FAIL("illegal regular expression");
+				if (np > 0) phi[np - 1] = hi;
+				continue;
+			}
+			if (o->nocase && is_upper(cc)) cc += 32;                   /* Pattern[] is lower-cased as a whole */
+			if (np < 2 * WIDTH) { plo[np] = phi[np] = cc; np++; }
+		}
+		if (regex && closed && np == 0) FAIL("illegal regular expression");
+		for (q = 0; q < np; q++) {
+			if (plo[q] == S_NOCARE) { cls_range(p, S_NOCARE, S_NOCARE); if (regex) cls_set(p, '\n'); }   /* maskgen.c:242-246 looks at the low end first: '.' = any */
+			else if (plo[q] <= phi[q]) cls_range(p, plo[q], phi[q]);
+		}
+	}
+	if (!closed) FAIL("unmatched '[', ']' (use \\[, \\] to search for [, ])");
+	if (compl_) { p->cls[0] = ~p->cls[0]; p->cls[1] = ~p->cls[1]; p->cls[2] = ~p->cls[2]; p->cls[3] = ~p->cls[3]; }
+	if (o->nocase) {                                                   /* maskgen.c:259-266: Mask[U] = Mask[u] */
+		int u;
+		memcpy(keep, p->cls, sizeof keep);
+		for (u = 'A'; u <= 'Z'; u++) {
+			p->cls[u >> 6] &= ~(1ull << (u & 63));
+			if (keep[(u + 32) >> 6] >> ((u + 32) & 63) & 1) cls_set(p, u);
+		}
+	}
+	*pi = i;
+	return 0;
+}
+
 /* the user's pattern (after the delimiter part and the optional -w/-x opener) */
 static int add_pattern(build_t *b, const unsigned char *s, int n, const agb_options *o, int L, char *err, size_t errlen)
 {
@@ -152,49 +202,9 @@ static int add_pattern(build_t *b, const unsigned char *s, int n, const agb_opti
 			if (b->no_error) p->prot = 1;
 			cls_range(p, S_NOCARE, S_NOCARE);
 			break; }
-		case S_LRANGE: {                                                       /* maskgen.c:96-127 */
-			pos_t *p = new_pos(b); int compl_ = 0, closed = 0, lo;
-			uint64_t keep[4];
-			if (!p) FAIL("pattern too long (has > %d chars)", WIDTH);
-			if (b->no_error) p->prot = 1;
-			i++;
-			if (i < n && s[i] == '^') { compl_ = 1; i++; }
-			lo = -1;
-			{   /* maskgen.c:104-116 keeps the class as (low, high) pairs: a symbol opens the pair (c, c), "-x" replaces the high
-			     * end of the last pair -- so a descending range like z-a matches nothing, not even z */
-				int plo[2 * WIDTH], phi[2 * WIDTH], np = 0, q;
-				for (; i < n; i++) {
-					int cc = map_sym(s, &i, n, 1, &esc);
-					if (!esc && cc == S_RRANGE) { closed = 1; break; }
-					if (!esc && cc == S_HYPHEN) {                              /* class[k-1] = next symbol */
-						int hi;
-						i++;
-						if (i >= n) break;
-						hi = map_sym(s, &i, n, 1, &esc);
-						if (o->nocase && is_upper(hi)) hi += 32;
-						if (np > 0) phi[np - 1] = hi;
-						continue;
-					}
-					if (o->nocase && is_upper(cc)) cc += 32;                   /* Pattern[] is lower-cased as a whole */
-					if (np < 2 * WIDTH) { plo[np] = phi[np] = cc; np++; }
-				}
-				for (q = 0; q < np; q++) {
-					if (plo[q] == S_NOCARE) cls_range(p, S_NOCARE, S_NOCARE);   /* maskgen.c:242-246 looks at the low end first: '.' = any */
-					else if (plo[q] <= phi[q]) cls_range(p, plo[q], phi[q]);
-				}
-			}
-			(void)lo;
-			if (!closed) FAIL("unmatched '[', ']' (use \\[, \\] to search for [, ])");
-			if (compl_) { p->cls[0] = ~p->cls[0]; p->cls[1] = ~p->cls[1]; p->cls[2] = ~p->cls[2]; p->cls[3] = ~p->cls[3]; }
-			if (o->nocase) {                                                   /* maskgen.c:259-266: Mask[U] = Mask[u] */
-				int u;
-				memcpy(keep, p->cls, sizeof keep);
-				for (u = 'A'; u <= 'Z'; u++) {
-					p->cls[u >> 6] &= ~(1ull << (u & 63));
-					if (keep[(u + 32) >> 6] >> ((u + 32) & 63) & 1) cls_set(p, u);
-				}
-			}
-			break; }
+		case S_LRANGE:
+			if (add_class(b, s, &i, n, o, 0, err, errlen)) return AGB_ERR_PATTERN;
+			break;
 		default:
 			if (add_literal(b, c, o->nocase, err, errlen)) return AGB_ERR_PATTERN;
 		}
@@ -507,7 +517,222 @@ static int parse_delim(const agb_options *o, build_t *b, agb_desc *d, char *err,
 	return 0;
 }
 
+/* ================================================================================================
+ * regular expressions (REGEX): the syntax of parse.c:181-237, the positions of maskgen.c, the follow sets of
+ * follow.c:210-255 as a Glushkov construction (first, last, nullable), in 64-bit words: up to 63 positions where the
+ * reference stops at 30 (preproce.c:378).  The pattern is wrapped as ".( ... )." (preproce.c:231-236, 334-339):
+ * position 1 is the leading '.', which the start state already holds (HEAD), position M the trailing one that the match
+ * test reads (bit 0).  '?' is the optional operator parse.c:220 means it to be (the reference also counts it as a
+ * literal position in maskgen(), so its bits no longer line up: SURVEY 8c).
+ * ============================================================================================== */
+typedef struct { uint64_t first, last; int nullable; } rx_frag;   /* sets of positions: bit p = position p */
+typedef struct {
+	build_t *b; const unsigned char *s; int i, n; const agb_options *o;
+	uint64_t fol[WIDTH + 1];                                     /* bit q of fol[p]: position q may follow p */
+	int and_seen;                                                /* a ';' was met (it never reaches parse(), preproce.c:308-311) */
+	char *err; size_t errlen;
+} rx_parser;
+
+/* an unescaped '|' or '*' makes the pattern a regular expression (preproce.c:139-142) */
+static int is_regex(const unsigned char *s, int m)
+{
+	int i;
+	for (i = 0; i < m; i++) {
+		if (s[i] == '\\') i++;
+		else if (s[i] == '|' || s[i] == '*') return 1;
+	}
+	return 0;
+}
+
+static void rx_link(rx_parser *P, uint64_t from, uint64_t to)
+{
+	int p;
+	for (p = 1; p < WIDTH; p++) if (from >> p & 1) P->fol[p] |= to;
+}
+
+static int rx_alt(rx_parser *P, rx_frag *out);
+
+static int rx_atom(rx_parser *P, rx_frag *f)
+{
+	build_t *b = P->b; const unsigned char *s = P->s; const int n = P->n;
+	char *err = P->err; size_t errlen = P->errlen;
+	int c = s[P->i];
+	pos_t *p;
+	if (c == '(') {
+		P->i++;
+		if (rx_alt(P, f)) return AGB_ERR_PATTERN;
+		if (P->i >= n || s[P->i] != ')') FAIL("illegal regular expression");
+		P->i++;
+		return 0;
+	}
+	if (c == '[') {
+		if (add_class(b, s, &P->i, n, P->o, 1, err, errlen)) return AGB_ERR_PATTERN;
+		P->i++;
+	} else if (c == '\\') {
+		if (P->i + 1 >= n) FAIL("illegal regular expression");
+		P->i++;
+		if (add_literal(b, s[P->i], P->o->nocase, err, errlen)) FAIL("regular expression too long");
+		P->i++;
+	} else if (c == '.' || c == '#') {                       /* '#' is ".*" under REGEX (preproce.c:247-253) */
+		if (!(p = new_pos(b))) FAIL("regular expression too long");
+		if (b->no_error) p->prot = 1;
+		cls_range(p, S_NOCARE, S_NOCARE); cls_set(p, '\n');  /* NOCARE takes '\n' too under REGEX (maskgen.c:243) */
+		P->i++;
+	} else if (c == '^' || c == '$') {                       /* a newline position (preproce.c:281-290) */
+		if (add_literal(b, '\n', 0, err, errlen)) FAIL("regular expression too long");
+		P->i++;
+	} else if (c == '*' || c == '?' || c == '|' || c == ')' || c == ']' || c == ',' || c == ';') {
+		FAIL("illegal regular expression");                  /* RE_ERR (preproce.c:299-306), or parse() fails */
+	} else {
+		if (c >= 129 && c <= 145) FAIL("byte %d in the pattern collides with an internal symbol (agrep.h:69-87)", c);
+		if (add_literal(b, c, P->o->nocase, err, errlen)) FAIL("regular expression too long");
+		P->i++;
+	}
+	f->first = f->last = 1ull << b->n;
+	f->nullable = 0;
+	if (c == '#') { rx_link(P, f->last, f->first); f->nullable = 1; }
+	return 0;
+}
+
+/* concatenation of starred / optional atoms; '<' '>' switch the error protection as elsewhere (maskgen.c:80-95) */
+static int rx_cat(rx_parser *P, rx_frag *out)
+{
+	build_t *b = P->b; const unsigned char *s = P->s;
+	char *err = P->err; size_t errlen = P->errlen;
+	int any = 0;
+	while (P->i < P->n && s[P->i] != '|' && s[P->i] != ')') {
+		rx_frag f;
+		if (s[P->i] == ';') { P->and_seen = 1; P->i++; continue; }
+		if (s[P->i] == '<') { b->no_error = 1; b->even++; P->i++; continue; }
+		if (s[P->i] == '>') { b->no_error = 0; if (--b->even < 0) FAIL("unmatched '<', '>' (use \\<, \\> to search for <, >)"); P->i++; continue; }
+		if (rx_atom(P, &f)) return AGB_ERR_PATTERN;
+		while (P->i < P->n && (s[P->i] == '*' || s[P->i] == '?')) {
+			if (s[P->i] == '*') rx_link(P, f.last, f.first);
+			f.nullable = 1;
+			P->i++;
+		}
+		if (!any) *out = f;
+		else {
+			rx_link(P, out->last, f.first);
+			out->first |= out->nullable ? f.first : 0;
+			out->last = f.last | (f.nullable ? out->last : 0);
+			out->nullable = out->nullable && f.nullable;
+		}
+		any = 1;
+	}
+	if (!any) FAIL("illegal regular expression");
+	return 0;
+}
+
+static int rx_alt(rx_parser *P, rx_frag *out)
+{
+	if (rx_cat(P, out)) return AGB_ERR_PATTERN;
+	while (P->i < P->n && P->s[P->i] == '|') {
+		rx_frag f;
+		P->i++;
+		if (rx_cat(P, &f)) return AGB_ERR_PATTERN;
+		out->first |= f.first; out->last |= f.last; out->nullable = out->nullable || f.nullable;
+	}
+	return 0;
+}
+
+uint64_t agbi_regex_next(const agb_regex *rx, int M, uint64_t S)
+{
+	uint64_t r = 0; int p;
+	for (p = 0; p <= M; p++) if (S >> (M - p) & 1) r |= rx->follow[p];
+	return r;
+}
+
+/* the rows right after a newline: Init[i] = Init[i-1] | Next(Init[i-1]) (agrep.c:1289), then the newline fed through
+ * every row (agrep.c:1649-1658).  Every line starts from them, the first one too (the virtual '\n' in front of the text) */
+static int rx_derive(agb_desc *d, const agb_regex *rx, char *err, size_t errlen)
+{
+	uint64_t B[AGB_MAXERR + 1], A[AGB_MAXERR + 1], m; int r, M = d->M;
+	if (d->engine != AGB_ENGINE_REGEX) FAIL("bad descriptor (not a regular expression)");
+	if (M < 2 || M > AGB_REGEX_MAXPOS) FAIL("regular expression too long");
+	if (d->k < 0 || d->k > 4) FAIL("the maximum number of erorrs allowed for full regular expressions is 4");   /* bitap.c:96-104 */
+	if (d->L != 1 || d->delim[0] != '\n') FAIL("-d or -w option is not supported for this pattern");
+	m = d->mask['\n'];
+	B[0] = d->init0;
+	for (r = 1; r <= d->k; r++) B[r] = B[r - 1] | agbi_regex_next(rx, M, B[r - 1]);
+	A[0] = (agbi_regex_next(rx, M, B[0]) & m) | (d->init1 & B[0]);
+	for (r = 1; r <= d->k; r++)
+		A[r] = (agbi_regex_next(rx, M, B[r]) & m) | (d->init1 & B[r]) | ((B[r - 1] | agbi_regex_next(rx, M, A[r - 1] | B[r - 1])) & d->noerr);
+	memset(d->reset, 0, sizeof d->reset); memset(d->start, 0, sizeof d->start);
+	memcpy(d->reset, A, sizeof(uint64_t) * (size_t)(d->k + 1));
+	memcpy(d->start, A, sizeof(uint64_t) * (size_t)(d->k + 1));
+	d->start_closes = 1;                         /* the virtual '\n' closes the (never reported) line in front of the text */
+	d->nrows = d->k + 1;
+	d->delim_kind = 0; memset(d->delim_fold, 0, sizeof d->delim_fold);
+	d->plan = AGB_PLAN_ALL; d->n_anchors = 0; d->n_anchors3 = 0; d->adaptive = 0; d->refine = 0;
+	return 0;
+}
+
+static int rx_build(const unsigned char *s, int m, const agb_options *o, agb_desc *d, agb_regex *rx, char *err, size_t errlen)
+{
+	rx_parser P; rx_frag u; build_t *b; pos_t *p; int M, q, c, rc = 0;
+	/* preproce.c:347-364, 378; compat.c:75-79 (-I/-S/-D are ignored, the command line says so) */
+	if (o->delim || o->wordbound) FAIL("-d or -w option is not supported for this pattern");
+	if (o->wholeline) FAIL("-x is not supported for regular expressions");
+	{   /* RE_ERR (preproce.c:299-311): any ',', or a second ';' */
+		int i, ors = 0, ands = 0;
+		for (i = 0; i < m; i++) {
+			if (s[i] == '\\') i++;
+			else if (s[i] == ',') ors++;
+			else if (s[i] == ';') ands++;
+		}
+		if (ors || ands > 1) FAIL("illegal regular expression");
+	}
+	b = (build_t *)calloc(1, sizeof *b);
+	if (!b) FAIL("out of memory");
+	memset(&P, 0, sizeof P);
+	P.b = b; P.s = s; P.i = 0; P.n = m; P.o = o; P.err = err; P.errlen = errlen;
+	p = new_pos(b);                                          /* the leading '.' */
+	cls_range(p, S_NOCARE, S_NOCARE); cls_set(p, '\n');
+	rc = rx_alt(&P, &u);
+	if (!rc && P.i < m) { rc = AGB_ERR_PATTERN; if (err && errlen) snprintf(err, errlen, "illegal regular expression"); }   /* an unmatched ')' */
+	if (!rc && b->even != 0) { rc = AGB_ERR_PATTERN; if (err && errlen) snprintf(err, errlen, "unmatched '<', '>' (use \\<, \\> to search for <, >)"); }
+	/* one ';' passes preprocess() and parse() and is refused by maskgen() (maskgen.c:150-163) */
+	if (!rc && P.and_seen) { rc = AGB_ERR_PATTERN; if (err && errlen) snprintf(err, errlen, "illegal pattern: cannot handle AND (';') and OR (',')/regular-expressions simultaneously"); }
+	if (!rc) {
+		p = new_pos(b);                                      /* the trailing '.' */
+		if (!p) { rc = AGB_ERR_PATTERN; if (err && errlen) snprintf(err, errlen, "regular expression too long"); }
+		else { cls_range(p, S_NOCARE, S_NOCARE); cls_set(p, '\n'); }
+	}
+	if (rc) { free(b); return rc; }
+	M = b->n;
+	P.fol[0] = 1ull << 1;
+	P.fol[1] |= u.first | (u.nullable ? 1ull << M : 0);
+	rx_link(&P, u.last, 1ull << M);
+	memset(rx, 0, sizeof *rx);
+	rx->head = 1; rx->tail = 1;
+	for (q = 0; q <= M; q++) {
+		int t;
+		for (t = 1; t <= M; t++) if (P.fol[q] >> t & 1) rx->follow[q] |= 1ull << (M - t);
+	}
+	/* the words (maskgen.c:218-257 under REGEX) */
+	d->M = M; d->engine = AGB_ENGINE_REGEX; d->k = o->k; d->inverse = o->inverse != 0;
+	d->cost_i = d->cost_s = d->cost_d = 1;
+	d->L = 1; d->delim[0] = '\n'; d->user_delim = 0; d->outtail = 0; d->and_mode = 0;
+	d->noerr = ~0ull; d->wildmask = 0; d->dmask = ~0ull; d->dendpos = 0; d->endpos = 1;
+	memset(d->mask, 0, sizeof d->mask);
+	for (q = 1; q <= M; q++) {
+		const pos_t *pq = &b->p[q];
+		if (pq->prot) d->noerr &= ~(1ull << (M - q));
+		for (c = 0; c < 256; c++) if (cls_has(pq, c)) d->mask[c] |= 1ull << (M - q);
+	}
+	d->init0 = (1ull << M) | (rx->head ? 1ull << (M - 1) : 0);   /* Init[0] = Bit[base] | Bit[base+1] (agrep.c:1285-1286) */
+	d->init1 = d->init0 | 1;
+	free(b);
+	return rx_derive(d, rx, err, errlen);
+}
+
 int agbi_build(const char *pattern, const agb_options *o, agb_desc *d, char *err, size_t errlen)
+{
+	return agbi_build_rx(pattern, o, d, NULL, err, errlen);
+}
+
+int agbi_build_rx(const char *pattern, const agb_options *o, agb_desc *d, agb_regex *rx, char *err, size_t errlen)
 {
 	build_t *b; int m, rc, notsgrep = 0, simple, jump, sg; unsigned char lut[256];
 	const unsigned char *s = (const unsigned char *)pattern;
@@ -520,6 +745,11 @@ int agbi_build(const char *pattern, const agb_options *o, agb_desc *d, char *err
 	if (m <= o->k) FAIL("size of pattern '%s' must be > #of errors %d", pattern, o->k);          /* checksg.c:34 */
 	if (o->wordbound && o->wholeline) FAIL("illegal option combination (-x and -w)");            /* agrep.c:2194 */
 	if (o->delim && o->wholeline) FAIL("-d and -x are not compatible");                          /* compat.c */
+	if (o->regex && is_regex(s, m)) {
+		/* the -B sweeps of this library (agb_bestmatch_*) rebuild the pattern at k = 2, 4, 8: not for re() */
+		if (!rx) FAIL("-B (best match) is not supported for regular expressions by the device sweep; scan with k = 0..4");
+		return rx_build(s, m, o, d, rx, err, errlen);
+	}
 	jump = (o->cost_i || o->cost_s || o->cost_d);
 	if (jump && (o->cost_i < 0 || o->cost_s < 0 || o->cost_d < 0)) FAIL("the error cost cannot be 0");
 	d->k = o->k; d->inverse = o->inverse != 0;
@@ -583,7 +813,28 @@ int agb_compile(const char *pattern, const agb_options *opt, agb_pattern **out, 
 	if (!out) return AGB_ERR_ARG;
 	p = (agb_pattern *)calloc(1, sizeof *p);
 	if (!p) return AGB_ERR_NOMEM;
-	rc = agbi_build(pattern, opt, &p->d, err, errlen);
+	rc = agbi_build_rx(pattern, opt, &p->d, &p->rx, err, errlen);
+	if (rc) { free(p); *out = NULL; return rc; }
+	*out = p;
+	return AGB_OK;
+}
+
+const agb_regex *agb_pattern_regex(const agb_pattern *p) { return (p && p->d.engine == AGB_ENGINE_REGEX) ? &p->rx : NULL; }
+
+int agb_pattern_from_regex(const agb_desc *d, const agb_regex *rx, agb_pattern **out, char *err, size_t errlen)
+{
+	agb_pattern *p; int rc, q;
+	if (err && errlen) err[0] = 0;
+	if (!d || !rx || !out) return AGB_ERR_ARG;
+	p = (agb_pattern *)calloc(1, sizeof *p);
+	if (!p) return AGB_ERR_NOMEM;
+	p->d = *d; p->rx = *rx;
+	/* nothing outside positions 0..M */
+	if (p->d.M >= 1 && p->d.M <= AGB_REGEX_MAXPOS) {
+		const uint64_t field = (p->d.M == 63) ? ~0ull : (2ull << p->d.M) - 1;
+		for (q = 0; q <= AGB_REGEX_MAXPOS; q++) p->rx.follow[q] = q <= p->d.M ? p->rx.follow[q] & field : 0;
+	}
+	rc = rx_derive(&p->d, &p->rx, err, errlen);
 	if (rc) { free(p); *out = NULL; return rc; }
 	*out = p;
 	return AGB_OK;

@@ -47,6 +47,7 @@ extern "C" void agb_shutdown(void)
 		cudaFree(W.tile_counts); cudaFree(W.tile_offsets); cudaFree(W.cand); cudaFree(W.cand_counts); cudaFree(W.cand_offsets);
 		cudaFree(W.cand_first); cudaFree(W.scan_sums); cudaFree(W.scan_offs); cudaFree(W.ord_blocks); cudaFree(W.totals);
 		cudaFreeHost(W.h_totals); cudaFree(W.d_desc); cudaFree(W.h2d_text); cudaFree(W.h2d_rec); cudaFree(W.d_gram); cudaFreeHost(W.h_gram);
+		cudaFree(W.d_regex);
 		if (W.e0) cudaEventDestroy(W.e0); if (W.e1) cudaEventDestroy(W.e1); if (W.e2) cudaEventDestroy(W.e2);
 		for (int i = 0; i < STAGE_BUFS; i++) { if (W.ev_copy[i]) cudaEventDestroy(W.ev_copy[i]); if (W.stage[i]) cudaFreeHost(W.stage[i]); }
 		if (W.s_copy) cudaStreamDestroy(W.s_copy); if (W.s_comp) cudaStreamDestroy(W.s_comp);
@@ -132,6 +133,23 @@ static int ws_upload_desc(Workspace &W, const agb_desc &d, cudaStream_t st)
 	return AGB_OK;
 }
 
+/* AGB_ENGINE_REGEX: the pattern's Next tables to the device (regex.cu reads them from RecParams.rx_tab) */
+static int regex_prepare(Workspace &W, const agb_desc &d, const agb_regex *rx, cudaStream_t st)
+{
+	if (d.engine != AGB_ENGINE_REGEX) return AGB_OK;
+	if (!rx) { snprintf(g_err, sizeof g_err, "a regular expression needs its follow sets (agb_pattern_from_regex)"); return AGB_ERR_ARG; }
+	if (!W.d_regex) CUDA_TRY(cudaMalloc(&W.d_regex, sizeof W.h_regex));
+	uint64_t tab[8 * 256];
+	const size_t bytes = regex_tables(d, *rx, tab);
+	if (bytes != W.regex_bytes || memcmp(tab, W.h_regex, bytes) != 0) {
+		CUDA_TRY(cudaMemcpyAsync(W.d_regex, tab, bytes, cudaMemcpyHostToDevice, st));
+		CUDA_TRY(cudaStreamSynchronize(st));     /* tab is on this stack */
+		memcpy(W.h_regex, tab, bytes); W.regex_bytes = bytes;
+	}
+	W.regex_tail = rx->tail;
+	return AGB_OK;
+}
+
 /* the ordered candidate list -> records: count launch (per-candidate counts, the first record of each kept), scan,
  * emit launch.  The list length lives on the device (totals[12]); every grid here is sized by the list's capacity. */
 static int list_stage(const agb_desc &d, Workspace &W, RecParams &P, bool want_list, cudaStream_t st)
@@ -170,8 +188,23 @@ static int records_launch(const agb_desc &d, Workspace &W, const void *d_text, u
 	P.records = d_records; P.capacity = capacity;
 	P.totals = W.totals; P.emit = 0; P.levels = (want & AGB_WANT_LEVELS) ? 1 : 0; P.want_level = want_level;
 	P.own_lo = sh ? sh->own_lo : INT64_MIN; P.own_hi = sh ? sh->own_hi : INT64_MAX; P.shard_last = sh ? sh->last : 1;
+	P.rx_tab = W.d_regex; P.rx_tail = W.regex_tail;
 	if (!tiles) return AGB_OK;
 	const bool want_list = (want & AGB_WANT_RECORDS) && capacity;
+	if (d.engine == AGB_ENGINE_REGEX) {
+		/* regular expressions: no anchor plan, every byte through re()'s recurrence in the tile form (regex.cu) */
+		P.tile_counts = W.tile_counts; P.tile_offsets = W.tile_offsets;
+		const uint64_t rtiles = (n + DENSE_TILE - 1) / DENSE_TILE;
+		if (launch_regex(d, P, (unsigned)rtiles, st)) return AGB_ERR_ARG;
+		CUDA_TRY(cudaGetLastError());
+		if (want_list) {
+			k_scan_tiles<<<1, 1024, 0, st>>>(W.tile_counts, W.tile_offsets, rtiles, nullptr); g_launches++;
+			P.emit = 1;
+			if (launch_regex(d, P, (unsigned)rtiles, st)) return AGB_ERR_ARG;
+			CUDA_TRY(cudaGetLastError());
+		}
+		return AGB_OK;
+	}
 	if (use_front && refined) {
 		int rc = ws_cand_reserve(W, std::max<size_t>(W.cand_hint + W.cand_hint / 4, (size_t)(n_chunks / 512) + 65536)); if (rc) return rc;
 		const unsigned ranges = W.refine_ctas * (REFINE_THREADS / 32);
@@ -423,7 +456,8 @@ static bool complement_usable(const agb_desc &d)
 }
 
 int scan_device_impl(const agb_desc &d_in, const void *d_text, uint64_t n, int want, int want_level,
-                     agb_record *d_records, uint64_t capacity, cudaStream_t st, agb_result *res, const ShardInfo *sh)
+                     agb_record *d_records, uint64_t capacity, cudaStream_t st, agb_result *res, const ShardInfo *sh,
+                     const agb_regex *rx)
 {
 	if (!res) return AGB_ERR_ARG;
 	memset(res, 0, sizeof *res);
@@ -469,6 +503,7 @@ int scan_device_impl(const agb_desc &d_in, const void *d_text, uint64_t n, int w
 		return AGB_OK;
 	}
 	rc = ws_upload_desc(W, d, st); if (rc) return rc;
+	rc = regex_prepare(W, d, rx, st); if (rc) return rc;
 	CUDA_TRY(cudaMemsetAsync(W.totals, 0, 16 * sizeof(unsigned long long), st));
 	CUDA_TRY(cudaEventRecord(W.e0, st));
 	bool use_front = front_usable(d) && n > 0;
@@ -488,7 +523,7 @@ extern "C" int agb_scan_device(const agb_pattern *p, const void *d_text, uint64_
                                agb_record *d_records, uint64_t capacity, void *stream, agb_result *res)
 {
 	if (!p) return AGB_ERR_ARG;
-	return scan_device_impl(p->d, d_text, n, want, -1, d_records, capacity, (cudaStream_t)stream, res);
+	return scan_device_impl(p->d, d_text, n, want, -1, d_records, capacity, (cudaStream_t)stream, res, nullptr, agb_pattern_regex(p));
 }
 
 static void par_memcpy(uint8_t *dst, const uint8_t *src, size_t len)
@@ -559,7 +594,7 @@ static bool read_slice(const SliceSource &src, int *dfd, uint64_t off, uint8_t *
 	return par_pread(src.fd, src.fd_off + (off_t)off, dst, len, false);
 }
 
-static int scan_stream_impl(const agb_desc &d, uint64_t n, const SliceSource &src, int want,
+static int scan_stream_impl(const agb_desc &d, const agb_regex *rx, uint64_t n, const SliceSource &src, int want,
                             agb_record *records, uint64_t capacity, agb_result *res)
 {
 	memset(res, 0, sizeof *res);
@@ -585,6 +620,7 @@ static int scan_stream_impl(const agb_desc &d, uint64_t n, const SliceSource &sr
 		CUDA_TRY(cudaMalloc(&W.h2d_rec, capacity * sizeof(agb_record))); W.h2d_rec_cap = capacity;
 	}
 	rc = ws_upload_desc(W, d, W.s_comp); if (rc) return rc;
+	rc = regex_prepare(W, d, rx, W.s_comp); if (rc) return rc;
 	const bool direct = src.mem && src.pinned;
 	FdGuard dg; if (!src.mem && src.fd >= 0) dg.fd = open_direct(src.fd, src.fd_off);
 	int &dfd = dg.fd;
@@ -645,7 +681,7 @@ extern "C" int agb_scan_host(const agb_pattern *p, const void *h_text, uint64_t 
 		src.pinned = cudaPointerGetAttributes(&attr, h_text) == cudaSuccess && attr.type == cudaMemoryTypeHost;
 		cudaGetLastError();
 	}
-	return scan_stream_impl(p->d, n, src, want, records, capacity, res);
+	return scan_stream_impl(p->d, agb_pattern_regex(p), n, src, want, records, capacity, res);
 }
 
 extern "C" int agb_scan_fd(const agb_pattern *p, int fd, int want, agb_record *records, uint64_t capacity, agb_result *res)
@@ -658,7 +694,7 @@ extern "C" int agb_scan_fd(const agb_pattern *p, int fd, int want, agb_record *r
 		off_t cur = lseek(fd, 0, SEEK_CUR);
 		uint64_t n = (cur >= 0 && sb.st_size > cur) ? (uint64_t)(sb.st_size - cur) : 0;
 		SliceSource src; src.mem = nullptr; src.pinned = false; src.fd = fd; src.fd_off = cur >= 0 ? cur : 0;
-		int rc = scan_stream_impl(p->d, n, src, want, records, capacity, res);
+		int rc = scan_stream_impl(p->d, agb_pattern_regex(p), n, src, want, records, capacity, res);
 		if (cur >= 0) lseek(fd, cur + (off_t)n, SEEK_SET);            /* as read(2) would have left it */
 		return rc;
 	}
@@ -751,7 +787,7 @@ extern "C" uint64_t agb_text_size(const agb_text *t) { return t ? t->n : 0; }
 extern "C" const void *agb_text_device(const agb_text *t) { return t ? t->d : nullptr; }
 
 /* device scan of a resident text with the record list delivered to host memory */
-static int scan_text_impl(const agb_desc &d, const agb_text *t, int want, int want_level, agb_record *records, uint64_t capacity, agb_result *res)
+static int scan_text_impl(const agb_desc &d, const agb_regex *rx, const agb_text *t, int want, int want_level, agb_record *records, uint64_t capacity, agb_result *res)
 {
 	if (!t || !res) return AGB_ERR_ARG;
 	if ((want & AGB_WANT_RECORDS) && capacity && !records) return AGB_ERR_ARG;
@@ -767,7 +803,7 @@ static int scan_text_impl(const agb_desc &d, const agb_text *t, int want, int wa
 		}
 		d_rec = W.h2d_rec;
 	}
-	int rc = scan_device_impl(d, t->d, t->n, want, want_level, d_rec, capacity, nullptr, res); if (rc) return rc;
+	int rc = scan_device_impl(d, t->d, t->n, want, want_level, d_rec, capacity, nullptr, res, nullptr, rx); if (rc) return rc;
 	if (res->n_records) CUDA_TRY(cudaMemcpy(records, d_rec, res->n_records * sizeof(agb_record), cudaMemcpyDeviceToHost));
 	return AGB_OK;
 }
@@ -775,7 +811,7 @@ static int scan_text_impl(const agb_desc &d, const agb_text *t, int want, int wa
 extern "C" int agb_scan_text(const agb_pattern *p, const agb_text *t, int want, agb_record *records, uint64_t capacity, agb_result *res)
 {
 	if (!p) return AGB_ERR_ARG;
-	return scan_text_impl(p->d, t, want, -1, records, capacity, res);
+	return scan_text_impl(p->d, agb_pattern_regex(p), t, want, -1, records, capacity, res);
 }
 
 /* keep the records of one level (stable, in place: the output index never overtakes the input index) */

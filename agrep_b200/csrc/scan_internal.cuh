@@ -4,6 +4,7 @@
  *   refine.cu   stage 1.5 k_refine           (local verification of anchor hits)
  *   records.cu  stage 2   k_records, k_records_dense, k_records_list
  *   slices.cu   stage 2   k_records_slices   (the automaton over every byte, in lockstep)
+ *   regex.cu    stage 2   k_regex            (regular expressions: re()'s recurrence over every byte, tile form)
  *   aux.cu      bitmap compaction, scans, density sample, ordinals, synthetic corpus
  *   scan.cu     workspace, orchestration, the C ABI (include/agrep_b200.h)
  * automaton.cuh holds the device pieces stages 1.5 and 2 share (the recurrence, the match test, the text reader). */
@@ -101,6 +102,8 @@ struct RecParams {
 	 * asearch.c:175-196); unsharded: everything.  shard_last = 0: the delimiter appended behind the text (bitap.c:161-165)
 	 * is not the text's own end -- an owned record that only it closes has outrun the halo (totals[11] is raised) */
 	int64_t own_lo, own_hi; int shard_last;
+	/* regular expressions (regex.cu): the byte-sliced Next tables on the device, TAIL's epsilon move at '\n' */
+	const void *rx_tab; int rx_tail;
 };
 struct ShardInfo { int64_t own_lo, own_hi; int last; };
 #define DENSE_THREADS 256
@@ -171,6 +174,8 @@ struct Workspace {               /* grow-only device scratch, one per device */
 	cudaStream_t s_copy = nullptr, s_comp = nullptr;
 	cudaEvent_t ev_copy[STAGE_BUFS] = {nullptr, nullptr, nullptr};
 	uint8_t *stage[STAGE_BUFS] = {nullptr, nullptr, nullptr};
+	/* the Next tables of the last regular expression scanned (regex.cu), and their host copy */
+	uint64_t *d_regex = nullptr; uint64_t h_regex[8 * 256]; size_t regex_bytes = 0; int regex_tail = 0;
 };
 
 /* scan.cu */
@@ -178,7 +183,8 @@ struct Workspace {               /* grow-only device scratch, one per device */
 extern Workspace g_ws[64];
 extern std::mutex g_ws_mu[64];   /* one scan at a time per device (the workspaces are shared scratch) */
 int  scan_device_impl(const agb_desc &d, const void *d_text, uint64_t n, int want, int want_level,
-                      agb_record *d_records, uint64_t capacity, cudaStream_t st, agb_result *res, const ShardInfo *sh = nullptr);
+                      agb_record *d_records, uint64_t capacity, cudaStream_t st, agb_result *res, const ShardInfo *sh = nullptr,
+                      const agb_regex *rx = nullptr);
 /* front.cu */
 bool front_usable(const agb_desc &d);
 bool exact_count_usable(const agb_desc &d);
@@ -196,6 +202,9 @@ int  launch_dense(const agb_desc &d, const RecParams &P, unsigned grid, cudaStre
 int  launch_records_list(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 int  launch_slices(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 bool slices_usable(const agb_desc &d);
+/* regex.cu: stage 2 of AGB_ENGINE_REGEX (RecParams.rx_tab set), and its tables (returns the bytes written: 32- or 64-bit words) */
+int  launch_regex(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
+size_t regex_tables(const agb_desc &d, const agb_regex &rx, uint64_t *out);
 /* aux.cu */
 __global__ void k_gram_sample(const uint8_t *text, uint64_t n_chunks, uint32_t nblk, uint32_t blk_chunks,
                               int ngram, const uint32_t *gram, const uint32_t *gmask, uint32_t fold, unsigned int *counts);

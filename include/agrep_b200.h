@@ -47,7 +47,8 @@ typedef struct agb_options {
 	int32_t ins_free;     /* -p  I = 0                                                       */
 	int32_t cost_i, cost_s, cost_d;   /* -I# -S# -D# ; 0 = not given                         */
 	int32_t bestmatch;    /* -B  BESTMATCH: forces the bitap family (checksg.c:127)          */
-	int32_t reserved;
+	int32_t regex;        /* 1: accept regular expressions (an unescaped '|' or '*', preproce.c:139-142) as
+	                         AGB_ENGINE_REGEX; 0: refuse them                                 */
 	const char *delim;    /* -d  argument as typed, NULL = newline records                   */
 } agb_options;
 
@@ -56,7 +57,8 @@ enum { AGB_ENGINE_BITAP = 0,    /* bitap.c:169-284   exact shift-and            
        AGB_ENGINE_ASEARCH = 1,  /* asearch.c:94-306  k = 1..4                                 */
        AGB_ENGINE_ASEARCH0 = 2, /* asearch.c:620-774 k = 5..8                                 */
        AGB_ENGINE_ASEARCH1 = 3, /* asearch1.c:86-235 non-unit costs                           */
-       AGB_ENGINE_SGREP_BM = 4  /* sgrep.c:262 + bm() sgrep.c:694: simple literal, k = 0      */ };
+       AGB_ENGINE_SGREP_BM = 4, /* sgrep.c:262 + bm() sgrep.c:694: simple literal, k = 0      */
+       AGB_ENGINE_REGEX = 5     /* re() agrep.c:1267-1917: regular expression, k = 0..4, lines */ };
 
 /* front-end plan chosen by agb_compile for the device scan */
 enum { AGB_PLAN_ALL = 0,        /* every 16-byte chunk goes to the record stage               */
@@ -103,6 +105,20 @@ typedef struct agb_desc {
 
 typedef struct agb_pattern agb_pattern;       /* opaque: agb_desc + bookkeeping              */
 
+/* What a regular expression adds to the descriptor (AGB_ENGINE_REGEX): the Glushkov automaton's follow sets.
+ * Positions are numbered as in the descriptor: position p at bit M-p; position 0 is the start state at bit M, which every
+ * state holds.  Next(S) = the union of follow[p] over the positions p of S (compute_next, agrep.c:396-457), so
+ * follow[0] is the start feed.  The descriptor of a regex pattern holds mask[] (Mask[], '.' matching '\n' too,
+ * maskgen.c:243), init0 (Init[0], with the HEAD position), init1 (Init0 | 1), noerr (NO_ERR_MASK), endpos = 1 (the
+ * trailing position of the ".( ... )." wrapper, preproce.c:231-236, 334-339), L = 1 with delim '\n' and k <= 4;
+ * reset[] = start[] = the rows after a newline.  Records are always lines. */
+#define AGB_REGEX_MAXPOS 63
+typedef struct agb_regex {
+	uint64_t follow[AGB_REGEX_MAXPOS + 1];    /* follow[p], p = 0..M                                */
+	int32_t  head, tail;                      /* HEAD / TAIL of preprocess(); tail: the epsilon move at '\n' (agrep.c:1332) */
+	int32_t  pad[2];
+} agb_regex;
+
 /* one matching record, in the reference's own terms (file offsets, not buffer indexes):
  *   begin   = offset of lasti: first byte of the delimiter that closed the previous record; -1 for the
  *             virtual '\n' in front of the text (bitap.c:140), 0 when a user delimiter has not been seen yet
@@ -141,6 +157,10 @@ const agb_desc *agb_pattern_desc(const agb_pattern *p);
 /* wrap words produced elsewhere (the drop-in layer passes the reference's globals); the plan fields are honoured
  * when plan == AGB_PLAN_ANCHORS, else every chunk goes to the record stage */
 int  agb_pattern_from_desc(const agb_desc *d, agb_pattern **out, char *err, size_t errlen);
+/* regular expressions: the follow sets of a pattern of AGB_ENGINE_REGEX (NULL for every other engine), and a pattern
+ * from words produced elsewhere (d->engine must be AGB_ENGINE_REGEX; reset[] and start[] are derived here) */
+const agb_regex *agb_pattern_regex(const agb_pattern *p);
+int  agb_pattern_from_regex(const agb_desc *d, const agb_regex *rx, agb_pattern **out, char *err, size_t errlen);
 
 /* ---- device scan ----
  * d_text: device pointer, 16-byte aligned, readable up to the next 16-byte boundary after n.
@@ -217,7 +237,8 @@ int  agb_bestmatch_sharded(const char *pattern, const agb_options *opt, agb_comm
  * A host walk over the delimiters, only needed for -n. */
 void agb_fill_ordinals(const agb_pattern *p, const void *h_text, uint64_t n, agb_record *records, uint64_t n_records);
 
-/* the -B sweep of agrep.c:3582-3728 in one pass for every best level up to 2 (at most three: k = 2, 4, 8): best_k =
+/* the -B sweep of agrep.c:3582-3728 in one pass for every best level up to 2 (at most three: k = 2, 4, 8; a regular
+ * expression is refused with AGB_ERR_PATTERN and a message -- the command line sweeps it level by level): best_k =
  * smallest level 0..min(M-1,8) at which a record matches (-1: none), res->n_matched = the records at that level (the
  * reference's "N words match within K errors"), d_records[0..res->n_records) = their ordered list (what the final
  * printing pass, agrep.c:3673-3726, prints); capacity 0: count only */

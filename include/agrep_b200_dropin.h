@@ -7,7 +7,7 @@
  *
  *   symbol      replaces (reference file:line)        what it does here
  *   ---------   ----------------------------------   ------------------------------------------------------
- *   bitap       bitap.c:78-448                        dispatcher + exact shift-and scan on the GPU; regex -> re()/re1()
+ *   bitap       bitap.c:78-448                        dispatcher + exact shift-and scan on the GPU; regex: re() on the GPU, re1()
  *   asearch     asearch.c:32-572                      k = 1..4 scan on the GPU
  *   asearch0    asearch.c:574-982                     k = 5..8 scan on the GPU
  *   asearch1    asearch1.c:28-435                     -I/-S/-D cost scan on the GPU
