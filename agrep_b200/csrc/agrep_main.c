@@ -18,7 +18,7 @@
 
 static const char *prog = "agrep-b200";
 static int COUNT, SILENT, FILENAMEONLY, NOFILENAME, LINENUM, BYTECOUNT, BESTMATCH, NOPROMPT, VERBOSE = 1, OUTTAIL;
-static int FNAME, num_of_matched, FIRSTOUTPUT = 1, EATFIRST;
+static int FNAME, num_of_matched, FIRSTOUTPUT = 1, EATFIRST, QUIET_OPEN;
 
 static void usage(void)
 {
@@ -39,7 +39,7 @@ static int is_regex(const char *s)
 static unsigned char *slurp(const char *path, size_t *n, int L, const unsigned char *dpat)
 {
 	int fd = path ? open(path, O_RDONLY) : 0; struct stat sb; size_t cap, len = 0; unsigned char *b;
-	if (fd < 0) { fprintf(stderr, "%s: can't open file for reading: %s\n", prog, path); return NULL; }
+	if (fd < 0) { if (!QUIET_OPEN) fprintf(stderr, "%s: can't open file for reading: %s\n", prog, path); return NULL; }
 	cap = (fstat(fd, &sb) == 0 && S_ISREG(sb.st_mode)) ? (size_t)sb.st_size + 1 : (1u << 20);
 	b = (unsigned char *)malloc(cap + 64);
 	if (!b) { if (path) close(fd); return NULL; }
@@ -84,8 +84,9 @@ static void print_record(const unsigned char *hb, const agb_desc *d, const agb_r
 	if (i1 <= i2) fwrite(hb + i1, 1, (size_t)(i2 - i1 + 1), stdout);
 }
 
-/* one pass of exec() over the files (agrep.c:3411-3576); counting = the COUNT=ON passes of the -B sweep */
-static int scan_files(const agb_pattern *p, char **files, int nfiles, int counting)
+/* one pass of exec() over the files (agrep.c:3411-3576); counting = the COUNT=ON passes of the -B sweep; hist (counting
+ * only): a levels pass -- every file's histogram of smallest levels is added to hist[] */
+static int scan_files(const agb_pattern *p, char **files, int nfiles, int counting, unsigned long long *hist)
 {
 	int fi;
 	for (fi = 0; fi < (nfiles ? nfiles : 1); fi++) {
@@ -100,12 +101,13 @@ static int scan_files(const agb_pattern *p, char **files, int nfiles, int counti
 		cap = count_only ? 0 : n / 64 + 65536;
 		for (;;) {
 			if (cap) { recs = (agb_record *)realloc(recs, cap * sizeof *recs); if (!recs) { fprintf(stderr, "%s: out of memory\n", prog); exit(255); } }
-			rc = agb_scan_host(p, hb + 1, n, count_only ? AGB_WANT_COUNT : (AGB_WANT_RECORDS | AGB_WANT_ORDINALS)   /* output() needs j even without -n (agrep.c:3815) */, recs, cap, &res);
+			rc = agb_scan_host(p, hb + 1, n, count_only ? (hist ? AGB_WANT_LEVELS : AGB_WANT_COUNT) : (AGB_WANT_RECORDS | AGB_WANT_ORDINALS)   /* output() needs j even without -n (agrep.c:3815) */, recs, cap, &res);
 			if (rc) { fprintf(stderr, "%s: scan failed: %s\n", prog, agb_last_error()); exit(255); }   /* no CPU fallback */
 			if (!res.truncated) break;
 			cap = (size_t)res.n_matched;
 		}
-		if (FILENAMEONLY && !counting) num_of_matched += res.n_matched ? 1 : 0;   /* the scan stops at the first hit (bitap.c:184-210, sgrep.c:813-814) */
+		if (hist) { for (i = 0; i <= AGB_MAXERR; i++) hist[i] += res.level_hist[i]; }
+		else if (FILENAMEONLY && !counting) num_of_matched += res.n_matched ? 1 : 0;   /* the scan stops at the first hit (bitap.c:184-210, sgrep.c:813-814) */
 		else if (count_only) num_of_matched += (int)res.n_matched;
 		else {
 			for (i = 0; i < res.n_records; i++) print_record(hb, d, &recs[i], fname ? fname : "");
@@ -117,6 +119,48 @@ static int scan_files(const agb_pattern *p, char **files, int nfiles, int counti
 		free(recs); free(hb);
 	}
 	return num_of_matched;
+}
+
+/* the counting passes of the -B sweep for a regular expression without -v.  The per-level sweep compiles and scans at
+ * k = 1, 2, ... up to `lim` (k < M, k <= AGB_MAXERR), stops at the first k that fails to compile, and at 4, the most a
+ * regular expression allows.  Here one count-only levels pass per file at k = min(2, top) gives every line's smallest
+ * level (re()'s rows are nested, so row j decides whether a line matches within j errors); only when no line has a level
+ * in 1..2 does a second pass at k = min(4, top) look at 3..4.  Returns the best level (-1: none) and sets num_of_matched to
+ * the lines at that level; stderr gets what the per-level sweep printed. */
+static int regex_best_level(const char *pattern, agb_options *o, char **files, int nfiles, int lim)
+{
+	unsigned long long hist[AGB_MAXERR + 1];
+	char err[256]; int k, top = 0, failed = 0, best = -1, lo = 1, passes, fi, l;
+	const int cap = lim < 4 ? lim : 4;
+	for (k = 1; k <= cap; k++) {
+		agb_pattern *pk; o->k = k;
+		if (agb_compile(pattern, o, &pk, err, sizeof err)) { failed = 1; break; }
+		agb_pattern_free(pk);
+		top = k;
+	}
+	QUIET_OPEN = 1;
+	while (best < 0 && lo <= top) {
+		agb_pattern *pk;
+		k = lo <= 2 && top > 2 ? 2 : top;
+		o->k = k;
+		if (agb_compile(pattern, o, &pk, err, sizeof err)) break;     /* compiled above */
+		memset(hist, 0, sizeof hist);
+		scan_files(pk, files, nfiles, 1, hist);
+		agb_pattern_free(pk);
+		for (l = lo; l <= k && best < 0; l++) if (hist[l]) best = l;
+		lo = k + 1;
+	}
+	QUIET_OPEN = 0;
+	/* the per-level sweep named every unreadable file once per pass: `best` passes, or one per level it tried */
+	passes = best > 0 ? best : top;
+	for (l = 0; l < passes; l++)
+		for (fi = 0; fi < nfiles; fi++) {
+			int fd = open(files[fi], O_RDONLY);
+			if (fd < 0) fprintf(stderr, "%s: can't open file for reading: %s\n", prog, files[fi]); else close(fd);
+		}
+	if (best < 0 && !failed && lim > 4) fprintf(stderr, "%s: no match within 4 errors, the most a regular expression allows\n", prog);
+	num_of_matched = best > 0 ? (int)hist[best] : 0;
+	return best;
 }
 
 int main(int argc, char **argv)
@@ -167,18 +211,20 @@ int main(int argc, char **argv)
 		return 255;
 	}
 
-	scan_files(p, argv + ai, nfiles, 0);
+	scan_files(p, argv + ai, nfiles, 0, NULL);
 	if (BESTMATCH && num_of_matched == 0 && nfiles > 0) {
 		/* agrep.c:3582-3728: nothing matched -> counting passes at D = 1, 2, ... < M, <= 8 until something matches,
-		 * report, ask (unless -y), then one printing pass at that D */
+		 * report, ask (unless -y), then one printing pass at that D.  A regular expression without -v takes its counting
+		 * passes from levels scans (regex_best_level) */
 		const int M = agb_pattern_desc(p)->M, regex = agb_pattern_desc(p)->engine == AGB_ENGINE_REGEX; int k, best = -1;
-		for (k = 1; k < M && k <= AGB_MAXERR && best < 0; k++) {
+		if (regex && !o.inverse) best = regex_best_level(pattern, &o, argv + ai, nfiles, M - 1 < AGB_MAXERR ? M - 1 : AGB_MAXERR);
+		else for (k = 1; k < M && k <= AGB_MAXERR && best < 0; k++) {
 			/* a regular expression allows 4 errors at most: the reference's sweep goes on to k = 5 and fails there (SURVEY 8c) */
 			if (regex && k > 4) { fprintf(stderr, "%s: no match within 4 errors, the most a regular expression allows\n", prog); break; }
 			agb_pattern *pk; o.k = k;
 			if (agb_compile(pattern, &o, &pk, err, sizeof err)) break;
 			num_of_matched = 0;
-			if (scan_files(pk, argv + ai, nfiles, 1) > 0) best = k;
+			if (scan_files(pk, argv + ai, nfiles, 1, NULL) > 0) best = k;
 			agb_pattern_free(pk);
 		}
 		if (best > 0) {
@@ -195,7 +241,7 @@ int main(int argc, char **argv)
 				agb_pattern_free(p); p = NULL; o.k = best;
 				if (agb_compile(pattern, &o, &p, err, sizeof err)) return 255;
 				num_of_matched = 0;
-				scan_files(p, argv + ai, nfiles, 0);
+				scan_files(p, argv + ai, nfiles, 0, NULL);
 			}
 		} else num_of_matched = 0;
 	}

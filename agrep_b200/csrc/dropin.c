@@ -23,6 +23,7 @@
  *     every file K + 2 times under -B (agrep.c:3582-3728), which then costs one upload, not K + 2;
  *   - under -B the counting passes D = 1, 2, ... are answered from ONE device pass that takes every record's
  *     smallest level (the rows are nested, asearch.c:98-114), and the final printing pass from the list that pass left;
+ *     for a re() pattern the counting passes come from levels passes at k = 2 and 4 (regex_bestmatch_count);
  *   - pipes, and memory mode (fd == -1, agrep.c:3282), go through a host buffer.
  */
 #define _GNU_SOURCE
@@ -415,12 +416,21 @@ done:
  * follow sets read from table[][] the way compute_next() reads them (agrep.c:405-415): positions 1 .. M-1, at most ten
  * entries each -- the reference's cap is kept on purpose here, the goal being its own output (SURVEY 8c).  Each matching
  * line goes through the reference's r_output() in a buffer of its own: '\n', the line, its newline. */
-static int regex_scan(int fd, int M, int D)
+static void regex_follow(int M, agb_regex *rx)
 {
-	agb_desc d; agb_regex rx; agb_pattern *p = NULL; agb_result res; agb_record *recs = NULL; source src;
-	unsigned char *buf = NULL; size_t bufcap = 0; unsigned long long i; int c, q, j, rc, ret = 0; char err[256];
-	const unsigned char nl = '\n';
-	memset(&d, 0, sizeof d); memset(&rx, 0, sizeof rx);
+	int q, j;
+	memset(rx, 0, sizeof *rx);
+	rx->follow[0] = 1ull << (M - 1);                         /* compute_next's constant k >> 1: the start feed */
+	for (q = 1; q < M; q++)
+		for (j = 0; j < 10 && table[q][j] > 0; j++) rx->follow[q] |= 1ull << (M - table[q][j]);
+	rx->head = HEAD; rx->tail = TAIL;
+}
+
+/* re()'s pattern at D errors from the globals; prints the error and returns -1 when the engine refuses it */
+static int regex_pattern(int M, int D, agb_pattern **p)
+{
+	agb_desc d; agb_regex rx; char err[256]; int c;
+	memset(&d, 0, sizeof d);
 	for (c = 0; c < 256; c++) d.mask[c] = Mask[c];
 	d.noerr = NO_ERR_MASK;
 	d.init0 = (1ull << M) | (HEAD ? 1ull << (M - 1) : 0);
@@ -428,14 +438,63 @@ static int regex_scan(int fd, int M, int D)
 	d.endpos = 1; d.dmask = ~0ull;
 	d.M = M; d.L = 1; d.delim[0] = '\n'; d.k = D; d.engine = AGB_ENGINE_REGEX; d.inverse = INVERSE;
 	d.cost_i = d.cost_s = d.cost_d = 1;
-	rx.follow[0] = 1ull << (M - 1);                          /* compute_next's constant k >> 1: the start feed */
-	for (q = 1; q < M; q++)
-		for (j = 0; j < 10 && table[q][j] > 0; j++) rx.follow[q] |= 1ull << (M - table[q][j]);
-	rx.head = HEAD; rx.tail = TAIL;
-	rc = agb_pattern_from_regex(&d, &rx, &p, err, sizeof err);
-	if (rc) { fprintf(stderr, "%s: %s\n", Progname, err); errno = AGREP_ERROR; return -1; }
-	source_open(fd, &src);
+	regex_follow(M, &rx);
+	if (agb_pattern_from_regex(&d, &rx, p, err, sizeof err)) { fprintf(stderr, "%s: %s\n", Progname, err); errno = AGREP_ERROR; return -1; }
+	return 0;
+}
+
+/* the -B memo key of a re() query: the words and follow sets regex_pattern() reads (-v never reaches the memo) */
+static unsigned long long bm_regex_signature(int M)
+{
+	unsigned long long h = 1469598103934665603ull; agb_regex rx; int c, q;
+#define MIX(x) do { h ^= (unsigned long long)(x); h *= 1099511628211ull; } while (0)
+	MIX(AGB_ENGINE_REGEX);
+	for (c = 0; c < 256; c++) MIX(Mask[c]);
+	MIX(NO_ERR_MASK); MIX(HEAD); MIX(TAIL); MIX(M);
+	regex_follow(M, &rx);
+	for (q = 0; q < M; q++) MIX(rx.follow[q]);
+#undef MIX
+	return h;
+}
+
+/* -B, the counting passes of a re() pattern (agrep.c:3591-3630, D = 1, 2, ... <= 4): the lines that match within D
+ * errors, from the file's memo of smallest levels.  re()'s rows are nested, so a levels pass at k = 2 answers D <= 2 and
+ * one at k = 4 the rest; each runs only when a D needs it. */
+static int regex_bestmatch_count(cache_entry *e, const source *s, int M, int D, unsigned long long *count)
+{
+	const unsigned long long sig = bm_regex_signature(M);
+	int l;
+	if (!e->bm_valid || e->bm_sig != sig) { e->bm_valid = 1; e->bm_sig = sig; e->bm_kdone = -1; e->bm_best = -1; memset(e->bm_hist, 0, sizeof e->bm_hist); free(e->bm_recs); e->bm_recs = NULL; e->bm_nrecs = 0; }
+	while (e->bm_kdone < D) {
+		agb_pattern *p = NULL; agb_result res; int rc, k = e->bm_kdone < 2 ? 2 : 4;
+		if (k < D) k = D;
+		if (regex_pattern(M, k, &p)) return -1;
+		rc = source_scan(p, s, AGB_WANT_LEVELS, NULL, 0, &res);
+		agb_pattern_free(p);
+		if (rc) return fail("scan");
+		for (l = e->bm_kdone + 1; l <= k; l++) e->bm_hist[l] = res.level_hist[l];
+		e->bm_kdone = k;
+	}
+	*count = 0;
+	for (l = 0; l <= D; l++) *count += e->bm_hist[l];
+	return 0;
+}
+
+static int regex_scan(int fd, int M, int D)
+{
+	agb_pattern *p = NULL; agb_result res; agb_record *recs = NULL; source src; cache_entry *ce;
+	unsigned char *buf = NULL; size_t bufcap = 0; unsigned long long i; int rc, ret = 0;
+	const unsigned char nl = '\n';
+	if (regex_pattern(M, D, &p)) return -1;
+	ce = source_open(fd, &src);
 	if (src.kind < 0) { agb_pattern_free(p); fprintf(stderr, "%s: out of memory\n", Progname); errno = AGREP_ERROR; return -1; }
+	if (BESTMATCH && COUNT && !FILENAMEONLY && D >= 1 && ce && !INVERSE) {
+		/* a counting pass of the -B sweep: answered from the levels memo of this file */
+		unsigned long long cnt = 0;
+		if (regex_bestmatch_count(ce, &src, M, D, &cnt)) ret = -1;
+		else num_of_matched += (int)cnt;
+		goto done;
+	}
 	if (COUNT && !FILENAMEONLY && fd != -1) {               /* r_output() would only count (agrep.c:1926-1927) */
 		rc = source_scan(p, &src, AGB_WANT_COUNT, NULL, 0, &res);
 		if (rc) ret = fail("scan");

@@ -15,7 +15,13 @@
  * 128-byte slice (the newline in front of them lies there) and walks them to their closing newline -- from shared
  * memory while the bytes are staged, from global memory after that, so a line of any length is finished by the
  * thread that owns it (serially: one thread per over-long line).  Count pass -> per-tile counts -> scan -> emit pass, as
- * k_records_dense; the emit launch recounts its tile before it writes, so a list walks every byte three times. */
+ * k_records_dense; the emit launch recounts its tile before it writes, so a list walks every byte three times.
+ *
+ * LEVELS (AGB_WANT_LEVELS): a line's level is the smallest row that passes the match test at its newline (records.cu's
+ * rule, -v included).  Row j depends on rows <= j only, so one pass at k yields every line's smallest level <= k.  The
+ * rows are nested (the reset rows are, and each step keeps it), so the test is monotone in the row: the last row (row 0
+ * under -v) is tested first and the other rows only behind a pass.  The extra work is per matching line; the count
+ * launch keeps a per-CTA histogram in shared memory and adds it to totals[2 + level] once. */
 #include "automaton.cuh"
 
 #define RX_THREADS 256
@@ -48,7 +54,16 @@ __device__ __forceinline__ void rx_step(T (&S)[NR], T cm, const T *tab, T init1,
 	S[NR - 1] = prevA;
 }
 
-template <typename T, int NR>
+/* the newline test of agrep.c:1614-1658 on one row */
+template <typename T>
+__device__ __forceinline__ bool rx_line_matches(T s, const T *tab, T mask_nl, T init1, bool tail, bool inverse)
+{
+	T t = (rx_next<T>(tab, s) & mask_nl) | (init1 & s);
+	if (tail) t |= rx_next<T>(tab, t);
+	return ((t & (T)1) != 0) != inverse;
+}
+
+template <typename T, int NR, bool LEVELS>
 __global__ void __launch_bounds__(RX_THREADS)
 k_regex(const RecParams P)
 {
@@ -57,6 +72,7 @@ k_regex(const RecParams P)
 	T *s_mask = s_tab + sizeof(T) * 256;                                   /* 256 */
 	uint8_t *s_text = reinterpret_cast<uint8_t *>(s_mask + 256);           /* RX_TILE + RX_TAIL */
 	__shared__ uint32_t s_scan[RX_THREADS];
+	__shared__ uint32_t s_hist[NR];                                        /* LEVELS: owned matching lines by level */
 	const uint32_t tid = threadIdx.x;
 	const agb_desc *D = P.desc;
 	const T *g_tab = reinterpret_cast<const T *>(P.rx_tab);
@@ -73,6 +89,7 @@ k_regex(const RecParams P)
 	T RS[NR];
 #pragma unroll
 	for (int r = 0; r < NR; r++) RS[r] = (T)D->reset[r];
+	if (LEVELS && tid < NR) s_hist[tid] = 0;
 	__syncthreads();
 	const T mask_nl = s_mask['\n'];
 	const uint32_t in_smem = (uint32_t)((int64_t)loaded < n - tile0 ? (int64_t)loaded : n - tile0);
@@ -131,15 +148,29 @@ k_regex(const RecParams P)
 				 * decided whatever the line's match, so that an owned line cut off by the end of a shard's halo is always
 				 * reported (rec_owned raises totals[11]) */
 				const bool counts = begin + 1 < n && rec_owned(P, begin, 1, p);
-				/* agrep.c:1614-1658: the match test on the last row, then the next line */
-				T t = (rx_next<T>(s_tab, S[NR - 1]) & mask_nl) | (init1 & S[NR - 1]);
-				if (tail) t |= rx_next<T>(s_tab, t);
-				const bool cond = ((t & (T)1) != 0) != inverse;
+				/* agrep.c:1614-1658: the match test on the last row (LEVELS: the smallest row that passes), then the next line */
+				int level = -1;
+				bool cond;
+				if constexpr (LEVELS) {
+					/* S[r] is a subset of S[r + 1] and the test is monotone in S, so without -v a line that fails the last
+					 * row fails them all, and with -v a row passes only if row 0 does: one test for most lines, as without
+					 * levels (a lane at its newline holds up its warp), the search only behind a pass */
+					if (rx_line_matches<T>(inverse ? S[0] : S[NR - 1], s_tab, mask_nl, init1, tail, inverse)) {
+						level = inverse ? 0 : NR - 1;
+						if (!inverse) {
+#pragma unroll
+							for (int r = 0; r < NR - 1; r++)
+								if (level == NR - 1 && rx_line_matches<T>(S[r], s_tab, mask_nl, init1, tail, false)) level = r;
+						}
+					}
+					cond = level >= 0;
+					if (cond && counts && !P.emit) atomicAdd(&s_hist[level], 1u);
+				} else cond = rx_line_matches<T>(S[NR - 1], s_tab, mask_nl, init1, tail, inverse);
 				if (cond && counts) {
 					if (pass == 1) {
 						const uint64_t at = out_pos + cnt;
 						if (at < P.capacity) {
-							agb_record rec; rec.begin = begin; rec.end = p; rec.ordinal = 0; rec.level = D->k; rec.pad = 0;
+							agb_record rec; rec.begin = begin; rec.end = p; rec.ordinal = 0; rec.level = LEVELS ? level : D->k; rec.pad = 0;
 							P.records[at] = rec;
 						}
 					}
@@ -167,6 +198,7 @@ k_regex(const RecParams P)
 					if (s_scan[RX_THREADS - 1]) atomicAdd(&P.totals[0], (unsigned long long)s_scan[RX_THREADS - 1]);
 					atomicAdd(&P.totals[1], (unsigned long long)((tile_len + 15) / 16));
 				}
+				if (LEVELS && tid < NR && s_hist[tid]) atomicAdd(&P.totals[2 + tid], (unsigned long long)s_hist[tid]);
 			} else out_pos = P.tile_offsets[blockIdx.x] + (s_scan[tid] - my_count);
 		}
 	}
@@ -174,27 +206,27 @@ k_regex(const RecParams P)
 
 template <typename T> static constexpr size_t rx_smem() { return sizeof(T) * 256 * sizeof(T) + 256 * sizeof(T) + RX_TILE + RX_TAIL; }
 
-template <typename T, int NR>
+template <typename T, int NR, bool LEVELS>
 static void launch_regex_one(const RecParams &P, unsigned grid, cudaStream_t st)
 {
 	static bool configured[64] = {false};
 	int dev = 0; cudaGetDevice(&dev);
 	if (!configured[dev & 63]) {
-		cudaFuncSetAttribute(k_regex<T, NR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rx_smem<T>());
+		cudaFuncSetAttribute(k_regex<T, NR, LEVELS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rx_smem<T>());
 		configured[dev & 63] = true;
 	}
-	k_regex<T, NR><<<grid, RX_THREADS, rx_smem<T>(), st>>>(P);
+	k_regex<T, NR, LEVELS><<<grid, RX_THREADS, rx_smem<T>(), st>>>(P);
 }
 
-template <typename T>
+template <typename T, bool LEVELS>
 static int launch_regex_t(int nrows, const RecParams &P, unsigned grid, cudaStream_t st)
 {
 	switch (nrows) {
-	case 1: launch_regex_one<T, 1>(P, grid, st); break;
-	case 2: launch_regex_one<T, 2>(P, grid, st); break;
-	case 3: launch_regex_one<T, 3>(P, grid, st); break;
-	case 4: launch_regex_one<T, 4>(P, grid, st); break;
-	case 5: launch_regex_one<T, 5>(P, grid, st); break;
+	case 1: launch_regex_one<T, 1, LEVELS>(P, grid, st); break;
+	case 2: launch_regex_one<T, 2, LEVELS>(P, grid, st); break;
+	case 3: launch_regex_one<T, 3, LEVELS>(P, grid, st); break;
+	case 4: launch_regex_one<T, 4, LEVELS>(P, grid, st); break;
+	case 5: launch_regex_one<T, 5, LEVELS>(P, grid, st); break;
 	default: return -1;
 	}
 	g_launches++;
@@ -207,7 +239,9 @@ bool regex_narrow(const agb_desc &d) { return d.M <= 31; }
 int launch_regex(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st)
 {
 	if (!P.rx_tab) return -1;
-	return regex_narrow(d) ? launch_regex_t<uint32_t>(d.nrows, P, grid, st) : launch_regex_t<uint64_t>(d.nrows, P, grid, st);
+	if (P.levels)
+		return regex_narrow(d) ? launch_regex_t<uint32_t, true>(d.nrows, P, grid, st) : launch_regex_t<uint64_t, true>(d.nrows, P, grid, st);
+	return regex_narrow(d) ? launch_regex_t<uint32_t, false>(d.nrows, P, grid, st) : launch_regex_t<uint64_t, false>(d.nrows, P, grid, st);
 }
 
 /* the byte-sliced Next tables of a regular expression, in the word width the kernel uses: slice s, byte value v ->

@@ -126,7 +126,8 @@ typedef struct agb_regex {
  *   ordinal = j at output() time; -n prints j-1 (agrep.c:3878); filled on the device when the scan is asked for
  *             AGB_WANT_ORDINALS (one more pass over the text that counts delimiters), else 0;
  *             agb_fill_ordinals() computes the same on a host copy of the text
- *   level   = smallest matching error level in best-match scans, else k                                */
+ *   level   = smallest matching error level in best-match and AGB_WANT_LEVELS scans (a regular expression's levels
+ *             come from an AGB_WANT_LEVELS scan), else k                                                   */
 typedef struct agb_record {
 	int64_t begin;
 	int64_t end;
@@ -238,7 +239,8 @@ int  agb_bestmatch_sharded(const char *pattern, const agb_options *opt, agb_comm
 void agb_fill_ordinals(const agb_pattern *p, const void *h_text, uint64_t n, agb_record *records, uint64_t n_records);
 
 /* the -B sweep of agrep.c:3582-3728 in one pass for every best level up to 2 (at most three: k = 2, 4, 8; a regular
- * expression is refused with AGB_ERR_PATTERN and a message -- the command line sweeps it level by level): best_k =
+ * expression is refused with AGB_ERR_PATTERN and a message -- its levels come from an AGB_WANT_LEVELS scan, which the
+ * command line runs at k = 2 and then 4): best_k =
  * smallest level 0..min(M-1,8) at which a record matches (-1: none), res->n_matched = the records at that level (the
  * reference's "N words match within K errors"), d_records[0..res->n_records) = their ordered list (what the final
  * printing pass, agrep.c:3673-3726, prints); capacity 0: count only */
