@@ -5,6 +5,8 @@ The reference exposes the scan path as `agrep [-# -i -w -x -v -n -p -I# -S# -D# 
 switches by name; `scan_*` return what exec() derives from the scan functions: num_of_matched and the
 (lasti, print_end, j) triples handed to output() (agrep.c:3805).  All work happens in libagrepb200.so."""
 import ctypes as C
+import os
+import stat
 from . import _lib
 from ._lib import (Options, Desc, Regex, Record, Result, CorpusSpec, WANT_COUNT, WANT_RECORDS, WANT_ORDINALS, WANT_LEVELS,
                    PLAN_ALL, PLAN_ANCHORS, ENGINE_NAMES, ENGINE_REGEX)
@@ -12,6 +14,12 @@ from ._lib import (Options, Desc, Regex, Record, Result, CorpusSpec, WANT_COUNT,
 
 class AgrepError(Exception):
     pass
+
+
+def _check_window(window):
+    """a window is a multiple of 512 bytes (the cut rule puts window edges on 512-byte blocks) and at least 4 KiB"""
+    if window is not None and (isinstance(window, bool) or not isinstance(window, int) or window < 4096 or window % 512):
+        raise ValueError("window must be a multiple of 512 and at least 4096 bytes, got %r" % (window,))
 
 
 class Pattern:
@@ -60,9 +68,12 @@ class Pattern:
         out = [(recs[i].begin, recs[i].end, recs[i].ordinal, recs[i].level) for i in range(res.n_records)] if recs is not None else []
         return res, out
 
-    def scan_host(self, data, want_records=True, capacity=None, levels=False, ordinals=False):
+    def scan_host(self, data, want_records=True, capacity=None, levels=False, ordinals=False, window=None):
         """data: bytes-like in host memory (the fill_buf path: H2D inside the call).
-        ordinals: also fill Record.ordinal (the j that -n prints) and Result.n_closes on the device."""
+        ordinals: also fill Record.ordinal (the j that -n prints) and Result.n_closes on the device.
+        window: None scans the whole text on the device (in windows only if it does not fit); a number of bytes (a
+        multiple of 512, >= 4096) keeps at most that much text, plus halos, on the device at a time -- same result."""
+        _check_window(window)
         n = len(data)
         want = (WANT_RECORDS if want_records else WANT_COUNT) | (WANT_LEVELS if levels else 0) | (WANT_ORDINALS if ordinals else 0)
         cap = (capacity if capacity is not None else n // 64 + 4096) if want_records else 0
@@ -70,10 +81,39 @@ class Pattern:
         while True:
             recs = (Record * cap)() if cap else None
             res = Result()
-            rc = _lib.lib().agb_scan_host(self._h, buf, n, want, recs, cap, C.byref(res))
+            if window is None:
+                rc = _lib.lib().agb_scan_host(self._h, buf, n, want, recs, cap, C.byref(res))
+            else:
+                rc = _lib.lib().agb_scan_host_windowed(self._h, buf, n, window, want, recs, cap, C.byref(res))
             if rc != 0 or not res.truncated or capacity is not None:
                 return self._finish(rc, res, recs, want)
             cap = res.n_matched          # the list did not fit (Result.truncated): once more with exactly n_matched entries
+
+    def scan_fd(self, fd, want_records=True, capacity=None, levels=False, ordinals=False, window=None):
+        """the text of file descriptor fd from its current offset to EOF (agb_scan_fd: regular files are pread(2) into
+        the pinned ring, pipes read into a host buffer); the offset is left at EOF.  window: as in scan_host.
+        Without a capacity the list is sized from the file's size and, when it did not fit, the file is scanned once
+        more from the same offset -- a pipe cannot be read twice, so there the truncated result is returned."""
+        _check_window(window)
+        start = None
+        try:
+            start = os.lseek(fd, 0, os.SEEK_CUR)
+            size = os.fstat(fd).st_size - start if stat.S_ISREG(os.fstat(fd).st_mode) else 0
+        except OSError:                  # a pipe
+            size = 0
+        want = (WANT_RECORDS if want_records else WANT_COUNT) | (WANT_LEVELS if levels else 0) | (WANT_ORDINALS if ordinals else 0)
+        cap = (capacity if capacity is not None else max(size, 0) // 64 + 4096) if want_records else 0
+        while True:
+            recs = (Record * cap)() if cap else None
+            res = Result()
+            if window is None:
+                rc = _lib.lib().agb_scan_fd(self._h, fd, want, recs, cap, C.byref(res))
+            else:
+                rc = _lib.lib().agb_scan_fd_windowed(self._h, fd, window, want, recs, cap, C.byref(res))
+            if rc != 0 or not res.truncated or capacity is not None or start is None:
+                return self._finish(rc, res, recs, want)
+            os.lseek(fd, start, os.SEEK_SET)
+            cap = res.n_matched
 
     def scan_device(self, dev_ptr, n, stream=0, d_records=0, capacity=0, levels=False, ordinals=False):
         """dev_ptr: device address of n bytes (16-byte aligned, e.g. torch tensor .data_ptr())."""

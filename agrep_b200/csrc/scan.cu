@@ -32,12 +32,14 @@ std::atomic<uint64_t> g_launches{0};
 extern "C" const char *agb_last_error(void) { return g_err; }
 extern "C" const char *agb_version(void) { return "agrep-b200 0.1 (sm_90a)"; }
 extern "C" uint64_t agb_kernel_launches(void) { return g_launches.load(); }
+static void win_release(int dev);
 /* frees the per-device scratch of this process (bitmaps, candidate lists, pinned rings, streams, events); the next
  * scan allocates again */
 extern "C" void agb_shutdown(void)
 {
 	int cur = 0; cudaGetDevice(&cur);
 	for (int dev = 0; dev < 64; dev++) {
+		win_release(dev);
 		std::lock_guard<std::mutex> lk(g_ws_mu[dev]);
 		Workspace &W = g_ws[dev];
 		if (!W.totals && !W.bitmap && !W.h2d_text) continue;
@@ -513,7 +515,7 @@ int scan_device_impl(const agb_desc &d_in, const void *d_text, uint64_t n, int w
 	if (use_front) { rc = front_launch(d, W, d_text, n, 0, ~0ull, false, st, count_in_front); if (rc) return rc; }
 	CUDA_TRY(cudaEventRecord(W.e1, st));
 	rc = stages_after_front(d, W, d_text, n, use_front, count_in_front, want, want_level, d_records, capacity, st, res, sh); if (rc) return rc;
-	if (sh && W.h_totals[11]) { snprintf(g_err, sizeof g_err, "a record of this shard runs past its halo (%d bytes behind the shard)", AGB_HALO_RIGHT); return AGB_ERR_ARG; }
+	/* (sh: a record that ran past the right halo raised totals[11]; shard_scan_geom reads it) */
 	CUDA_TRY(cudaEventElapsedTime(&res->ms_front, W.e0, W.e1));
 	CUDA_TRY(cudaEventElapsedTime(&res->ms_records, W.e1, W.e2));
 	return AGB_OK;
@@ -594,6 +596,17 @@ static bool read_slice(const SliceSource &src, int *dfd, uint64_t off, uint8_t *
 	return par_pread(src.fd, src.fd_off + (off_t)off, dst, len, false);
 }
 
+/* AGB_MAX_TEXT_BYTES: the most bytes of text the library keeps on the device (0 or unset: no cap) */
+static uint64_t max_text_bytes(void)
+{
+	const char *e = getenv("AGB_MAX_TEXT_BYTES");
+	return (e && *e) ? strtoull(e, nullptr, 10) : 0;
+}
+
+/* scan_stream_impl: the whole text does not fit on the device (cudaErrorMemoryAllocation, or more than AGB_MAX_TEXT_BYTES);
+ * the caller scans it in windows instead */
+#define SCAN_NEEDS_WINDOWS 1
+
 static int scan_stream_impl(const agb_desc &d, const agb_regex *rx, uint64_t n, const SliceSource &src, int want,
                             agb_record *records, uint64_t capacity, agb_result *res)
 {
@@ -602,17 +615,21 @@ static int scan_stream_impl(const agb_desc &d, const agb_regex *rx, uint64_t n, 
 	if (dev < 0 || dev >= 64) return AGB_ERR_ARG;
 	std::lock_guard<std::mutex> lk(g_ws_mu[dev]);
 	Workspace &W = g_ws[dev];
+	const size_t need = (size_t)((n + 15) / 16 * 16 + 4096);
+	const uint64_t cap_bytes = max_text_bytes();
+	if (need > W.h2d_cap || (cap_bytes && need > cap_bytes)) {
+		if (W.h2d_text) cudaFree(W.h2d_text);
+		W.h2d_text = nullptr; W.h2d_cap = 0;
+		if (cap_bytes && need > cap_bytes) return SCAN_NEEDS_WINDOWS;
+		const cudaError_t e = cudaMalloc(&W.h2d_text, need);
+		if (e == cudaErrorMemoryAllocation) { cudaGetLastError(); W.h2d_text = nullptr; return SCAN_NEEDS_WINDOWS; }
+		CUDA_TRY(e); W.h2d_cap = need;
+	}
 	int rc = ws_prepare(W, n); if (rc) return rc;
 	if (!W.s_copy) {
 		CUDA_TRY(cudaStreamCreateWithFlags(&W.s_copy, cudaStreamNonBlocking));
 		CUDA_TRY(cudaStreamCreateWithFlags(&W.s_comp, cudaStreamNonBlocking));
 		for (int i = 0; i < STAGE_BUFS; i++) CUDA_TRY(cudaEventCreateWithFlags(&W.ev_copy[i], cudaEventDisableTiming));
-	}
-	const size_t need = (size_t)((n + 15) / 16 * 16 + 4096);
-	if (need > W.h2d_cap) {
-		if (W.h2d_text) cudaFree(W.h2d_text);
-		W.h2d_text = nullptr; W.h2d_cap = 0;
-		CUDA_TRY(cudaMalloc(&W.h2d_text, need)); W.h2d_cap = need;
 	}
 	if ((want & AGB_WANT_RECORDS) && capacity > W.h2d_rec_cap) {
 		if (W.h2d_rec) cudaFree(W.h2d_rec);
@@ -670,21 +687,227 @@ static int scan_stream_impl(const agb_desc &d, const agb_regex *rx, uint64_t n, 
 	return AGB_OK;
 }
 
-extern "C" int agb_scan_host(const agb_pattern *p, const void *h_text, uint64_t n, int want,
-                             agb_record *records, uint64_t capacity, agb_result *res)
+/* ------------------------------------------------------------------------------------------------
+ * texts larger than the device's memory: the text in windows (DESIGN 3.4).  Window i owns the bytes [a_i, a_i + w) and is
+ * scanned as a shard of the whole text (shard.cu): from hl bytes before it to hr bytes behind it, the cut rule deciding
+ * which records are its own.  Two device buffers: while window i is scanned on the compute stream, a host thread moves
+ * window i + 1 (halos included: the bytes it shares with window i are uploaded again) through the pinned ring on the copy
+ * stream.  A window whose last record runs past hr, or whose left halo starts inside a run of the delimiter, is scanned
+ * again with that halo doubled -- in a buffer of its own -- until it is long enough or the range reaches the text's end.
+ * Counts and histograms are summed; each window's records are made global on the device and appended to the caller's
+ * list until it is full; the ordinals follow the gather's arithmetic (agb_shard_part).
+ * ---------------------------------------------------------------------------------------------- */
+struct WinState {                 /* per device, kept across calls: streams and the pinned ring (device buffers live for one call) */
+	cudaStream_t s_copy = nullptr, s_comp = nullptr;
+	cudaEvent_t ev[STAGE_BUFS] = {nullptr, nullptr, nullptr};
+	uint8_t *stage[STAGE_BUFS] = {nullptr, nullptr, nullptr};
+};
+static WinState g_win[64];
+static std::mutex g_win_mu[64];   /* one windowed scan at a time per device; taken before (never inside) g_ws_mu */
+
+static void win_release(int dev)
+{
+	std::lock_guard<std::mutex> lk(g_win_mu[dev]);
+	WinState &S = g_win[dev];
+	if (!S.s_copy) return;
+	if (cudaSetDevice(dev) != cudaSuccess) { cudaGetLastError(); return; }
+	cudaStreamSynchronize(S.s_copy); cudaStreamSynchronize(S.s_comp);
+	for (int i = 0; i < STAGE_BUFS; i++) { if (S.ev[i]) cudaEventDestroy(S.ev[i]); if (S.stage[i]) cudaFreeHost(S.stage[i]); }
+	cudaStreamDestroy(S.s_copy); cudaStreamDestroy(S.s_comp);
+	S = WinState();
+}
+
+/* device memory of one windowed scan */
+struct WinBuffers {
+	uint8_t *buf[2] = {nullptr, nullptr}, *big = nullptr; size_t big_cap = 0;
+	agb_record *rec = nullptr; uint64_t rec_cap = 0;
+	~WinBuffers() { cudaFree(buf[0]); cudaFree(buf[1]); cudaFree(big); cudaFree(rec); }
+};
+
+#define WIN_SLACK 4096            /* zeroed bytes behind a window's scanned range, as behind a whole text */
+
+/* bytes [lo, hi) of the source to dst on the device, then WIN_SLACK zero bytes; returns once they are there */
+static int upload_range(const SliceSource &src, int *dfd, WinState &S, uint64_t lo, uint64_t hi, uint8_t *dst)
+{
+	const bool direct = src.mem && src.pinned;
+	uint64_t i = 0;
+	for (uint64_t off = lo; off < hi; off += H2D_SLICE, i++) {
+		const uint64_t len = std::min<uint64_t>(H2D_SLICE, hi - off);
+		const int sb = (int)(i % STAGE_BUFS);
+		if (direct) { CUDA_TRY(cudaMemcpyAsync(dst + (off - lo), src.mem + off, len, cudaMemcpyHostToDevice, S.s_copy)); continue; }
+		if (i >= STAGE_BUFS) CUDA_TRY(cudaEventSynchronize(S.ev[sb]));          /* that staging buffer has been consumed */
+		if (src.mem) {
+			if (len < (1u << 20)) memcpy(S.stage[sb], src.mem + off, len);     /* (small windows: four threads cost more than they save) */
+			else par_memcpy(S.stage[sb], src.mem + off, len);
+		} else if (!read_slice(src, dfd, off, S.stage[sb], (size_t)len)) {
+			cudaStreamSynchronize(S.s_copy);
+			snprintf(g_err, sizeof g_err, "pread(2) failed or hit the end of the file in [%llu, %llu)", (unsigned long long)off, (unsigned long long)(off + len));
+			return AGB_ERR_ARG;
+		}
+		CUDA_TRY(cudaMemcpyAsync(dst + (off - lo), S.stage[sb], len, cudaMemcpyHostToDevice, S.s_copy));
+		CUDA_TRY(cudaEventRecord(S.ev[sb], S.s_copy));
+	}
+	CUDA_TRY(cudaMemsetAsync(dst + (hi - lo), 0, WIN_SLACK, S.s_copy));
+	CUDA_TRY(cudaStreamSynchronize(S.s_copy));
+	return AGB_OK;
+}
+
+/* window i with halos of (at most) hl and hr bytes */
+struct WinGeom { uint64_t a, n_local, hl, hr, lo, hi; bool first, open_end, reaches_end; };
+static WinGeom win_geom(uint64_t n, uint64_t w, uint64_t i, uint64_t hl, uint64_t hr)
+{
+	WinGeom g;
+	const uint64_t m = n ? (n + w - 1) / w : 1;
+	g.a = i * w; g.n_local = std::min<uint64_t>(w, n - g.a);
+	g.hl = i ? std::min<uint64_t>(hl, g.a) : 0;                       /* a, w and hl are multiples of 512: so is the clamp */
+	g.hr = std::min<uint64_t>(hr, n - g.a - g.n_local);
+	g.lo = g.a - g.hl; g.hi = g.a + g.n_local + g.hr;
+	g.first = i == 0; g.open_end = i + 1 == m; g.reaches_end = g.hi >= n;
+	return g;
+}
+
+static int scan_windowed(const agb_desc &d, const agb_regex *rx, uint64_t n, const SliceSource &src, uint64_t w, int want,
+                         agb_record *records, uint64_t capacity, agb_result *res)
+{
+	memset(res, 0, sizeof *res);
+	int dev = 0; CUDA_TRY(cudaGetDevice(&dev));
+	if (dev < 0 || dev >= 64) return AGB_ERR_ARG;
+	std::lock_guard<std::mutex> lk(g_win_mu[dev]);
+	WinState &S = g_win[dev];
+	if (!S.s_copy) {
+		CUDA_TRY(cudaStreamCreateWithFlags(&S.s_copy, cudaStreamNonBlocking));
+		CUDA_TRY(cudaStreamCreateWithFlags(&S.s_comp, cudaStreamNonBlocking));
+		for (int i = 0; i < STAGE_BUFS; i++) CUDA_TRY(cudaEventCreateWithFlags(&S.ev[i], cudaEventDisableTiming));
+	}
+	if (!(src.mem && src.pinned) && n && !S.stage[0]) for (int i = 0; i < STAGE_BUFS; i++) CUDA_TRY(cudaMallocHost(&S.stage[i], H2D_SLICE));
+	const bool want_list = (want & AGB_WANT_RECORDS) && capacity, ord = (want & AGB_WANT_ORDINALS) != 0;
+	WinBuffers B;
+	const size_t buf_bytes = std::min<uint64_t>(n, w + AGB_HALO_LEFT + AGB_HALO_RIGHT) + WIN_SLACK;
+	for (int b = 0; b < 2; b++) CUDA_TRY(cudaMalloc(&B.buf[b], buf_bytes));
+	if (want_list) {
+		/* most windows own far fewer records than bytes; one that owns more is scanned again with a longer list */
+		B.rec_cap = std::min<uint64_t>(capacity, w / 256 + 4096);
+		CUDA_TRY(cudaMalloc(&B.rec, B.rec_cap * sizeof(agb_record)));
+	}
+	FdGuard dg; if (!src.mem && src.fd >= 0) dg.fd = open_direct(src.fd, src.fd_off);
+	int &dfd = dg.fd;
+	const uint64_t m = n ? (n + w - 1) / w : 1;
+	int rc = upload_range(src, &dfd, S, 0, win_geom(n, w, 0, AGB_HALO_LEFT, AGB_HALO_RIGHT).hi, B.buf[0]); if (rc) return rc;
+	uint64_t copied = 0; long long origin = 0, closes_before = 0;
+	for (uint64_t i = 0; i < m; i++) {
+		/* the next window on its way while this one is scanned (the thread has the pinned ring and dfd to itself until joined) */
+		int up_rc = AGB_OK; char up_err[sizeof g_err] = "";
+		std::thread up;
+		struct Joiner { std::thread &t; ~Joiner() { if (t.joinable()) t.join(); } } joiner{up};   /* every way out of this iteration */
+		if (i + 1 < m) {
+			const WinGeom gn = win_geom(n, w, i + 1, AGB_HALO_LEFT, AGB_HALO_RIGHT);
+			uint8_t *dst = B.buf[(i + 1) & 1];
+			up = std::thread([&, gn, dst] {
+				up_rc = cudaSetDevice(dev) == cudaSuccess ? upload_range(src, &dfd, S, gn.lo, gn.hi, dst) : AGB_ERR_CUDA;
+				if (up_rc) memcpy(up_err, g_err, sizeof up_err);     /* (g_err is per thread) */
+			});
+		}
+		auto join_up = [&]() -> int {
+			if (up.joinable()) up.join();
+			if (up_rc) { memcpy(g_err, up_err, sizeof up_err); return up_rc; }
+			return AGB_OK;
+		};
+		uint64_t hl = AGB_HALO_LEFT, hr = AGB_HALO_RIGHT;
+		const uint8_t *base = B.buf[i & 1];
+		WinGeom g; agb_result lres; agb_shard_part part;
+		for (;;) {
+			g = win_geom(n, w, i, hl, hr);
+			const uint64_t room = want_list ? std::min<uint64_t>(capacity - copied, B.rec_cap) : 0;
+			rc = shard_window_scan(d, rx, base + g.hl, g.n_local, g.hl, g.hr, g.first, g.open_end, g.reaches_end, want,
+			                       B.rec, room, S.s_comp, &lres, &part);
+			if (rc < 0) return rc;
+			int short_halos = rc;
+			if (g.lo == 0) short_halos &= ~HALO_SHORT_LEFT;      /* the scan starts where the text does: a run there really begins there */
+			if (!short_halos) {
+				if (!(want_list && lres.n_matched > room && room < capacity - copied)) break;
+				/* more records than the list had room for, and the caller's list has more: again with room for all of them */
+				cudaFree(B.rec); B.rec = nullptr;
+				B.rec_cap = std::min<uint64_t>(capacity - copied, lres.n_matched);
+				CUDA_TRY(cudaMalloc(&B.rec, B.rec_cap * sizeof(agb_record)));
+				continue;
+			}
+			if (short_halos & HALO_SHORT_LEFT) hl *= 2;
+			if (short_halos & HALO_SHORT_RIGHT) hr *= 2;
+			g = win_geom(n, w, i, hl, hr);
+			rc = join_up(); if (rc) return rc;                      /* the ring is needed here */
+			const size_t need = g.hi - g.lo + WIN_SLACK;
+			if (need > B.big_cap) {
+				cudaFree(B.big); B.big = nullptr; B.big_cap = 0;
+				const cudaError_t e = cudaMalloc(&B.big, need);
+				if (e != cudaSuccess) {
+					cudaGetLastError();
+					snprintf(g_err, sizeof g_err, "a record that begins in bytes [%llu, %llu) of the text does not fit in device memory with its halos (%llu bytes: %s)",
+					         (unsigned long long)g.a, (unsigned long long)(g.a + g.n_local), (unsigned long long)need, cudaGetErrorString(e));
+					return e == cudaErrorMemoryAllocation ? AGB_ERR_NOMEM : AGB_ERR_CUDA;
+				}
+				B.big_cap = need;
+			}
+			rc = upload_range(src, &dfd, S, g.lo, g.hi, B.big); if (rc) return rc;
+			base = B.big;
+		}
+		res->n_matched += lres.n_matched; res->n_flagged += lres.n_flagged;
+		for (int l = 0; l <= AGB_MAXERR; l++) res->level_hist[l] += lres.level_hist[l];
+		res->ms_front += lres.ms_front; res->ms_records += lres.ms_records;
+		if (ord && i == 0) { origin = part.ord_origin; res->n_closes += (uint64_t)part.virt; }
+		if (lres.n_records) {
+			/* offsets: local to the scanned range, which starts at g.lo = g.a + part.byte_base; ordinals as the gather makes them */
+			rc = shard_window_rebase(B.rec, lres.n_records, (long long)g.a + part.byte_base, origin + closes_before - part.ord_fix, ord, S.s_comp);
+			if (rc) return rc;
+			CUDA_TRY(cudaMemcpyAsync(records + copied, B.rec, lres.n_records * sizeof(agb_record), cudaMemcpyDeviceToHost, S.s_comp));
+			CUDA_TRY(cudaStreamSynchronize(S.s_comp));
+			copied += lres.n_records;
+		}
+		if (ord) { closes_before += (long long)part.closes; res->n_closes += part.closes; }
+		rc = join_up(); if (rc) return rc;
+	}
+	res->n_records = copied;
+	res->truncated = ((want & AGB_WANT_RECORDS) && res->n_matched > capacity) ? 1 : 0;
+	return AGB_OK;
+}
+
+/* the window of a text that does not fit: two windows and their halos in what AGB_MAX_TEXT_BYTES allows, and in three
+ * quarters of the device's free memory less 512 MiB (the rest: the workspace of a window -- bitmaps, ordinal blocks and
+ * candidate list, about 4 % of it -- and its record list) */
+static uint64_t fallback_window(void)
+{
+	uint64_t budget = max_text_bytes();
+	size_t fr = 0, tot = 0;
+	if (cudaMemGetInfo(&fr, &tot) == cudaSuccess) {
+		const uint64_t usable = fr > (512ull << 20) ? (fr - (512ull << 20)) / 4 * 3 : 0;
+		if (!budget || usable < budget) budget = usable;
+	} else cudaGetLastError();
+	const uint64_t per = AGB_HALO_LEFT + AGB_HALO_RIGHT + WIN_SLACK;
+	return budget / 2 >= per + 4096 ? (budget / 2 - per) & ~(uint64_t)511 : 4096;
+}
+
+static bool host_pinned(const void *h_text, uint64_t n)
+{
+	if (!n) return false;
+	cudaPointerAttributes attr; memset(&attr, 0, sizeof attr);
+	const bool pinned = cudaPointerGetAttributes(&attr, h_text) == cudaSuccess && attr.type == cudaMemoryTypeHost;
+	cudaGetLastError();
+	return pinned;
+}
+
+/* window_bytes == 0: the whole text on the device when it fits, windows when it does not */
+static int scan_host_any(const agb_pattern *p, const void *h_text, uint64_t n, uint64_t window_bytes, int want,
+                         agb_record *records, uint64_t capacity, agb_result *res)
 {
 	if (!p || !res || (!h_text && n)) return AGB_ERR_ARG;
 	if ((want & AGB_WANT_RECORDS) && capacity && !records) return AGB_ERR_ARG;
-	SliceSource src; src.mem = (const uint8_t *)h_text; src.fd = -1; src.pinned = false;
-	if (n) {
-		cudaPointerAttributes attr; memset(&attr, 0, sizeof attr);
-		src.pinned = cudaPointerGetAttributes(&attr, h_text) == cudaSuccess && attr.type == cudaMemoryTypeHost;
-		cudaGetLastError();
-	}
-	return scan_stream_impl(p->d, agb_pattern_regex(p), n, src, want, records, capacity, res);
+	SliceSource src; src.mem = (const uint8_t *)h_text; src.fd = -1; src.pinned = host_pinned(h_text, n);
+	if (window_bytes) return scan_windowed(p->d, agb_pattern_regex(p), n, src, window_bytes, want, records, capacity, res);
+	int rc = scan_stream_impl(p->d, agb_pattern_regex(p), n, src, want, records, capacity, res);
+	if (rc == SCAN_NEEDS_WINDOWS) rc = scan_windowed(p->d, agb_pattern_regex(p), n, src, fallback_window(), want, records, capacity, res);
+	return rc;
 }
 
-extern "C" int agb_scan_fd(const agb_pattern *p, int fd, int want, agb_record *records, uint64_t capacity, agb_result *res)
+static int scan_fd_any(const agb_pattern *p, int fd, uint64_t window_bytes, int want, agb_record *records, uint64_t capacity, agb_result *res)
 {
 	if (!p || !res) return AGB_ERR_ARG;
 	if ((want & AGB_WANT_RECORDS) && capacity && !records) return AGB_ERR_ARG;
@@ -694,7 +917,9 @@ extern "C" int agb_scan_fd(const agb_pattern *p, int fd, int want, agb_record *r
 		off_t cur = lseek(fd, 0, SEEK_CUR);
 		uint64_t n = (cur >= 0 && sb.st_size > cur) ? (uint64_t)(sb.st_size - cur) : 0;
 		SliceSource src; src.mem = nullptr; src.pinned = false; src.fd = fd; src.fd_off = cur >= 0 ? cur : 0;
-		int rc = scan_stream_impl(p->d, agb_pattern_regex(p), n, src, want, records, capacity, res);
+		int rc = window_bytes ? scan_windowed(p->d, agb_pattern_regex(p), n, src, window_bytes, want, records, capacity, res)
+		                      : scan_stream_impl(p->d, agb_pattern_regex(p), n, src, want, records, capacity, res);
+		if (rc == SCAN_NEEDS_WINDOWS) rc = scan_windowed(p->d, agb_pattern_regex(p), n, src, fallback_window(), want, records, capacity, res);
 		if (cur >= 0) lseek(fd, cur + (off_t)n, SEEK_SET);            /* as read(2) would have left it */
 		return rc;
 	}
@@ -708,9 +933,41 @@ extern "C" int agb_scan_fd(const agb_pattern *p, int fd, int want, agb_record *r
 		if (r == 0) break;
 		len += (size_t)r;
 	}
-	int rc = agb_scan_host(p, buf, len, want, records, capacity, res);
+	int rc = scan_host_any(p, buf, len, window_bytes, want, records, capacity, res);
 	free(buf);
 	return rc;
+}
+
+extern "C" int agb_scan_host(const agb_pattern *p, const void *h_text, uint64_t n, int want,
+                             agb_record *records, uint64_t capacity, agb_result *res)
+{
+	return scan_host_any(p, h_text, n, 0, want, records, capacity, res);
+}
+
+extern "C" int agb_scan_fd(const agb_pattern *p, int fd, int want, agb_record *records, uint64_t capacity, agb_result *res)
+{
+	return scan_fd_any(p, fd, 0, want, records, capacity, res);
+}
+
+static bool window_ok(uint64_t w)
+{
+	if (w >= 4096 && w % 512 == 0) return true;
+	snprintf(g_err, sizeof g_err, "window_bytes (%llu) must be a multiple of 512 and at least 4096", (unsigned long long)w);
+	return false;
+}
+
+extern "C" int agb_scan_host_windowed(const agb_pattern *p, const void *h_text, uint64_t n, uint64_t window_bytes, int want,
+                                      agb_record *records, uint64_t capacity, agb_result *res)
+{
+	if (!window_ok(window_bytes)) return AGB_ERR_ARG;
+	return scan_host_any(p, h_text, n, window_bytes, want, records, capacity, res);
+}
+
+extern "C" int agb_scan_fd_windowed(const agb_pattern *p, int fd, uint64_t window_bytes, int want,
+                                    agb_record *records, uint64_t capacity, agb_result *res)
+{
+	if (!window_ok(window_bytes)) return AGB_ERR_ARG;
+	return scan_fd_any(p, fd, window_bytes, want, records, capacity, res);
 }
 
 /* ---- a text kept in HBM across scans (the drop-in layer's exec() scans the same file K + 2 times under -B,
@@ -721,8 +978,14 @@ static int text_upload(const SliceSource &src, uint64_t n, agb_text **out)
 {
 	int dev = 0; CUDA_TRY(cudaGetDevice(&dev));
 	if (dev < 0 || dev >= 64) return AGB_ERR_ARG;
-	agb_text *t = new agb_text; t->d = nullptr; t->n = n; t->dev = dev;
 	const size_t need = (size_t)((n + 15) / 16 * 16 + 4096);
+	const uint64_t cap_bytes = max_text_bytes();
+	if (cap_bytes && need > cap_bytes) {
+		snprintf(g_err, sizeof g_err, "a text of %llu bytes does not fit in AGB_MAX_TEXT_BYTES=%llu; agb_scan_host and agb_scan_fd scan it in windows",
+		         (unsigned long long)n, (unsigned long long)cap_bytes);
+		return AGB_ERR_NOMEM;
+	}
+	agb_text *t = new agb_text; t->d = nullptr; t->n = n; t->dev = dev;
 	if (cudaMalloc(&t->d, need) != cudaSuccess) { delete t; snprintf(g_err, sizeof g_err, "cudaMalloc of %zu bytes for the text failed", need); cudaGetLastError(); return AGB_ERR_NOMEM; }
 	std::lock_guard<std::mutex> lk(g_ws_mu[dev]);
 	Workspace &W = g_ws[dev];
@@ -778,7 +1041,8 @@ extern "C" int agb_text_from_fd(int fd, agb_text **out)
 	const uint64_t n = (cur >= 0 && sb.st_size > cur) ? (uint64_t)(sb.st_size - cur) : 0;
 	SliceSource src; src.mem = nullptr; src.pinned = false; src.fd = fd; src.fd_off = cur >= 0 ? cur : 0;
 	int rc = text_upload(src, n, out);
-	if (cur >= 0) lseek(fd, cur + (off_t)n, SEEK_SET);                /* as read(2) would have left it */
+	/* as read(2) would have left it; untouched when the text was not taken, so that the caller can read it another way */
+	if (cur >= 0) lseek(fd, rc == AGB_OK ? cur + (off_t)n : cur, SEEK_SET);
 	return rc;
 }
 

@@ -185,6 +185,13 @@ extern std::mutex g_ws_mu[64];   /* one scan at a time per device (the workspace
 int  scan_device_impl(const agb_desc &d, const void *d_text, uint64_t n, int want, int want_level,
                       agb_record *d_records, uint64_t capacity, cudaStream_t st, agb_result *res, const ShardInfo *sh = nullptr,
                       const agb_regex *rx = nullptr);
+/* shard.cu: one window of the windowed scan -- the shard scan, with a halo that is too short reported as a positive code
+ * (a set of HALO_SHORT_*) instead of an error; and the window's records made global on the device */
+enum { HALO_SHORT_RIGHT = 1, HALO_SHORT_LEFT = 2 };
+int  shard_window_scan(const agb_desc &d, const agb_regex *rx, const void *d_win, uint64_t n_local, uint64_t halo_left, uint64_t halo_right,
+                       bool first, bool open_end, bool reaches_end, int want, agb_record *d_records, uint64_t capacity,
+                       cudaStream_t st, agb_result *lres, agb_shard_part *part);
+int  shard_window_rebase(agb_record *d_records, uint64_t n, long long byte_add, long long ord_add, bool ordinals, cudaStream_t st);
 /* front.cu */
 bool front_usable(const agb_desc &d);
 bool exact_count_usable(const agb_desc &d);

@@ -242,11 +242,13 @@ static int comm_buffers(agb_comm *c, uint64_t local_cap, uint64_t pad_cap)
 
 /* the local part: this shard with its halos as one text, ownership by the cut rule.  first: nothing in front of the
  * shard (own range open to the left); open_end: nothing owned by anyone else behind it (own range open to the right);
- * reaches_end: the scanned bytes end where the whole text ends */
+ * reaches_end: the scanned bytes end where the whole text ends.
+ * grow: a halo that is too short is not an error but a request for a longer one -- the result and part are filled and
+ * the return value is HALO_SHORT_RIGHT and/or HALO_SHORT_LEFT (the windowed scan of scan.cu rescans with it doubled) */
 static int shard_scan_geom(const agb_desc &d, const void *d_shard, uint64_t n_local, uint64_t halo_left, uint64_t halo_right,
                            bool first, bool open_end, bool reaches_end, int want, int want_level,
                            agb_record *d_records, uint64_t capacity, cudaStream_t st, agb_result *lres, agb_shard_part *part,
-                           const agb_regex *rx = nullptr)
+                           const agb_regex *rx = nullptr, bool grow = false)
 {
 	if (((uintptr_t)d_shard & 15) || (halo_left & 15)) { snprintf(g_err, sizeof g_err, "shard pointer and left halo must be 16-byte aligned"); return AGB_ERR_ARG; }
 	if ((!first && (halo_left % 512)) || (!open_end && ((halo_left + n_local) % 512))) { snprintf(g_err, sizeof g_err, "shard boundaries must fall on multiples of 512 bytes of the scanned range"); return AGB_ERR_ARG; }
@@ -265,7 +267,9 @@ static int shard_scan_geom(const agb_desc &d, const void *d_shard, uint64_t n_lo
 	std::lock_guard<std::mutex> lk(g_ws_mu[dev]);
 	Workspace &W = g_ws[dev];
 	const bool ord = (want & AGB_WANT_ORDINALS) != 0;
-	if (W.h_totals[18]) { snprintf(g_err, sizeof g_err, "a run of the delimiter longer than the left halo (%llu bytes) crosses the start of this shard", (unsigned long long)halo_left); return AGB_ERR_ARG; }
+	const int short_halos = (W.h_totals[11] ? HALO_SHORT_RIGHT : 0) | (W.h_totals[18] ? HALO_SHORT_LEFT : 0);
+	if (!grow && W.h_totals[11]) { snprintf(g_err, sizeof g_err, "a record of this shard runs past its halo (%d bytes behind the shard)", AGB_HALO_RIGHT); return AGB_ERR_ARG; }
+	if (!grow && W.h_totals[18]) { snprintf(g_err, sizeof g_err, "a run of the delimiter longer than the left halo (%llu bytes) crosses the start of this shard", (unsigned long long)halo_left); return AGB_ERR_ARG; }
 	part->byte_base = -(int64_t)halo_left;
 	if (ord) {
 		const unsigned long long total = lres->n_closes - (unsigned long long)W.ord_virt;     /* delimiter ends the local scan saw */
@@ -276,6 +280,27 @@ static int shard_scan_geom(const agb_desc &d, const void *d_shard, uint64_t n_lo
 		part->ord_origin = first ? (long long)W.ord_virt + W.ord_j0 : 0;
 		part->virt = first ? W.ord_virt : 0;
 	}
+	return grow ? short_halos : AGB_OK;
+}
+
+/* one window of the windowed scan (scan.cu, scan_windowed): the shard scan in grow mode, then the window's records made
+ * global on the device -- begin/end += byte_add, ordinal += ord_add -- by the gather kernel over a world of one */
+int shard_window_scan(const agb_desc &d, const agb_regex *rx, const void *d_win, uint64_t n_local, uint64_t halo_left, uint64_t halo_right,
+                      bool first, bool open_end, bool reaches_end, int want, agb_record *d_records, uint64_t capacity,
+                      cudaStream_t st, agb_result *lres, agb_shard_part *part)
+{
+	return shard_scan_geom(d, d_win, n_local, halo_left, halo_right, first, open_end, reaches_end, want, -1, d_records, capacity, st,
+	                       lres, part, rx, true);
+}
+
+int shard_window_rebase(agb_record *d_records, uint64_t n, long long byte_add, long long ord_add, bool ordinals, cudaStream_t st)
+{
+	if (!n) return AGB_OK;
+	GatherParams G; memset(&G, 0, sizeof G);
+	G.world = 1; G.pad = n; G.count[0] = n; G.out_off[0] = 0; G.byte_base[0] = byte_add; G.ord_add[0] = ord_add; G.ordinals = ordinals ? 1 : 0;
+	dim3 grid((unsigned)std::min<uint64_t>((n + 255) / 256, 1024), 1);
+	k_gather_compact<<<grid, 256, 0, st>>>(d_records, d_records, n, G); g_launches++;     /* in place: every thread reads, then writes, its own entry */
+	CUDA_TRY(cudaGetLastError());
 	return AGB_OK;
 }
 

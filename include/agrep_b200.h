@@ -172,16 +172,36 @@ int  agb_scan_device(const agb_pattern *p, const void *d_text, uint64_t n, int w
                      agb_record *d_records, uint64_t capacity, void *stream, agb_result *res);
 
 /* host text: staged through pinned buffers in slices cut at record boundaries, H2D overlapped with the
- * scan (the fill_buf replacement, bitap.c:450-477).  records: host array. */
+ * scan (the fill_buf replacement, bitap.c:450-477).  records: host array.
+ * A text that does not fit on the device -- its buffer fails with cudaErrorMemoryAllocation, or it is larger than the
+ * environment's AGB_MAX_TEXT_BYTES -- is scanned in windows, as by agb_scan_host_windowed, with the same result.  The
+ * window then is the largest multiple of 512 such that two windows and their halos fit in AGB_MAX_TEXT_BYTES and in three
+ * quarters of the device's free memory less 512 MiB (DESIGN 3.4). */
 int  agb_scan_host(const agb_pattern *p, const void *h_text, uint64_t n, int want,
                    agb_record *records, uint64_t capacity, agb_result *res);
 
-/* file descriptor: read(2) loop into the pinned ring, as agb_scan_host */
+/* file descriptor: read(2) loop into the pinned ring, as agb_scan_host (windows included).  Starts at the current offset
+ * and leaves it at EOF; regular files are pread(2) by four threads (AGB_ODIRECT=1: past the page cache), pipes are read
+ * into a host buffer first */
 int  agb_scan_fd(const agb_pattern *p, int fd, int want, agb_record *records, uint64_t capacity, agb_result *res);
+
+/* as agb_scan_host / agb_scan_fd, but at most window_bytes of text (plus halos) is in device memory at a time; the
+ * result -- n_matched, level_hist, n_closes, the ordered list with global offsets and ordinals, truncated -- is what
+ * the whole-text scan returns.  window_bytes: a multiple of 512, >= 4096.  Each window is scanned as a shard of the
+ * whole text (the cut rule of agb_scan_shard_local) while the next one is uploaded; a halo that turns out too short (a
+ * record running past the right one, a run of the delimiter longer than the left one) is doubled and the window scanned
+ * again, so only a record that does not fit in device memory with its halos is an error (AGB_ERR_NOMEM, naming where
+ * it begins).  n_flagged, ms_front and ms_records are sums over the windows. */
+int  agb_scan_host_windowed(const agb_pattern *p, const void *h_text, uint64_t n, uint64_t window_bytes, int want,
+                            agb_record *records, uint64_t capacity, agb_result *res);
+int  agb_scan_fd_windowed(const agb_pattern *p, int fd, uint64_t window_bytes, int want,
+                          agb_record *records, uint64_t capacity, agb_result *res);
 
 /* ---- a text kept in HBM across scans ----
  * exec() scans the same file up to K + 2 times under -B (agrep.c:3582-3728); the drop-in layer uploads it once.
- * agb_text_from_fd: regular files, from the current offset to EOF, read(2) straight into the pinned ring. */
+ * agb_text_from_fd: regular files, from the current offset to EOF, read(2) straight into the pinned ring; the offset is
+ * left at EOF, or where it was when the call fails.  A text larger than AGB_MAX_TEXT_BYTES (environment) is refused with
+ * AGB_ERR_NOMEM: scan it with agb_scan_host / agb_scan_fd, which use windows. */
 typedef struct agb_text agb_text;
 int  agb_text_from_host(const void *h_text, uint64_t n, agb_text **out);
 int  agb_text_from_fd(int fd, agb_text **out);
