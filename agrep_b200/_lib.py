@@ -36,7 +36,7 @@ class Desc(C.Structure):
                 ("anchor", C.c_uint32 * AGB_MAXANCHOR), ("anchor_fold", C.c_uint32), ("anchor_mask", C.c_uint32),
                 ("refine", C.c_int32), ("pat_len", C.c_int32), ("anchor_off", C.c_int32 * AGB_MAXANCHOR),
                 ("n_anchors3", C.c_int32), ("anchor3", C.c_uint32 * 4), ("anchor3_off", C.c_int32 * 4), ("adaptive", C.c_int32),
-                ("delim_fold", C.c_uint8 * (2 * AGB_MAXDELIM + 2)), ("pad_", C.c_uint8 * 2)]
+                ("delim_fold", C.c_uint8 * (2 * AGB_MAXDELIM + 2)), ("pair_plan", C.c_uint8), ("pad_", C.c_uint8)]
 
 
 class Regex(C.Structure):

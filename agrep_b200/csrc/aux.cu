@@ -5,9 +5,30 @@
 
 /* how often does each candidate gram of the pattern start in a chunk?  One thread per 16-byte chunk of a sample of
  * the text (nblk stretches of blk_chunks chunks, evenly spread); the anchor planner (scan.cu) picks the k+1 disjoint
- * grams with the fewest hits: stage 1.5's work is proportional to the chunks stage 1 flags */
+ * grams with the fewest hits: stage 1.5's work is proportional to the chunks stage 1 flags.  n_pair > 0: grams
+ * [pair_first, pair_first + n_pair) are the pieces of a pair plan, and counts[127] gets the chunks its rule flags (some
+ * piece starts in the chunk, another one in it or in the next chunk) */
+__device__ __forceinline__ void sample_windows(const uint8_t *text, uint64_t chunk, uint32_t fold, uint32_t (&wv)[16])
+{
+	const uint4 v = __ldg(reinterpret_cast<const uint4 *>(text) + chunk);
+	const uint32_t x4 = __ldg(reinterpret_cast<const uint32_t *>(text) + (chunk + 1) * 4);
+	const uint32_t x[5] = { v.x | fold, v.y | fold, v.z | fold, v.w | fold, x4 | fold };
+#pragma unroll
+	for (int w = 0; w < 4; w++) {
+		wv[4 * w] = x[w]; wv[4 * w + 1] = __funnelshift_r(x[w], x[w + 1], 8);
+		wv[4 * w + 2] = __funnelshift_r(x[w], x[w + 1], 16); wv[4 * w + 3] = __funnelshift_r(x[w], x[w + 1], 24);
+	}
+}
+__device__ __forceinline__ bool sample_hit(const uint32_t (&wv)[16], uint32_t G, uint32_t M)
+{
+	bool hit = false;
+#pragma unroll
+	for (int s = 0; s < 16; s++) hit = hit || ((wv[s] & M) == G);
+	return hit;
+}
 __global__ void __launch_bounds__(256) k_gram_sample(const uint8_t *text, uint64_t n_chunks, uint32_t nblk, uint32_t blk_chunks,
-                                                    int ngram, const uint32_t *gram, const uint32_t *gmask, uint32_t fold, unsigned int *counts)
+                                                    int ngram, const uint32_t *gram, const uint32_t *gmask, uint32_t fold, unsigned int *counts,
+                                                    int pair_first, int n_pair)
 {
 	__shared__ unsigned int s_cnt[128];
 	if (threadIdx.x < 128) s_cnt[threadIdx.x] = 0;
@@ -17,26 +38,24 @@ __global__ void __launch_bounds__(256) k_gram_sample(const uint8_t *text, uint64
 	if (b < nblk) {
 		const uint64_t chunk = (n_chunks / nblk) * b + i;
 		if (chunk + 2 < n_chunks) {
-			const uint4 v = __ldg(reinterpret_cast<const uint4 *>(text) + chunk);
-			const uint32_t x4 = __ldg(reinterpret_cast<const uint32_t *>(text) + (chunk + 1) * 4);
-			const uint32_t x[5] = { v.x | fold, v.y | fold, v.z | fold, v.w | fold, x4 | fold };
 			uint32_t wv[16];
-#pragma unroll
-			for (int w = 0; w < 4; w++) {
-				wv[4 * w] = x[w]; wv[4 * w + 1] = __funnelshift_r(x[w], x[w + 1], 8);
-				wv[4 * w + 2] = __funnelshift_r(x[w], x[w + 1], 16); wv[4 * w + 3] = __funnelshift_r(x[w], x[w + 1], 24);
-			}
+			sample_windows(text, chunk, fold, wv);
+			uint32_t here = 0;                                   /* pair plan: its pieces that start in this chunk */
 			for (int g = 0; g < ngram; g++) {
-				const uint32_t G = gram[g], M = gmask[g];
-				bool hit = false;
-#pragma unroll
-				for (int s = 0; s < 16; s++) hit = hit || ((wv[s] & M) == G);
-				if (hit) atomicAdd(&s_cnt[g], 1u);
+				if (!sample_hit(wv, gram[g], gmask[g])) continue;
+				if (g < 127) atomicAdd(&s_cnt[g], 1u);
+				if (g >= pair_first && g < pair_first + n_pair) here |= 1u << (g - pair_first);
+			}
+			if (here) {
+				uint32_t next = 0;
+				sample_windows(text, chunk + 1, fold, wv);
+				for (int p = 0; p < n_pair; p++) if (sample_hit(wv, gram[pair_first + p], gmask[pair_first + p])) next |= 1u << p;
+				if (__popc(here | next) >= 2) atomicAdd(&s_cnt[127], 1u);
 			}
 		}
 	}
 	__syncthreads();
-	if (threadIdx.x < ngram && s_cnt[threadIdx.x]) atomicAdd(&counts[threadIdx.x], s_cnt[threadIdx.x]);
+	if (threadIdx.x < 128 && s_cnt[threadIdx.x]) atomicAdd(&counts[threadIdx.x], s_cnt[threadIdx.x]);
 }
 
 /* how dense are the flags?  popcount of every `stride`-th bitmap word (an estimate is all the host needs to pick the

@@ -68,6 +68,27 @@ __device__ __forceinline__ uint32_t windows_test(uint32_t lo, uint32_t hi, const
 	return acc;
 }
 
+/* -n: the delimiter bytes of chunk idx of the stage (SWAR: 0x80 where a byte equals the delimiter); summed over a warp
+ * they make one 512-byte block of the ordinals pass (aux.cu), which then need not read the text again */
+template <bool FULL>
+__device__ __forceinline__ uint32_t chunk_delims(const FrontParams &P, const uint4 v, uint32_t idx, uint32_t rem)
+{
+	const uint32_t xs[4] = { v.x, v.y, v.z, v.w };
+	uint32_t cn = 0;
+#pragma unroll
+	for (int w = 0; w < 4; w++) {
+		const uint32_t t = (xs[w] | P.dfold4) ^ P.delim4;
+		uint32_t z = ~(((t & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | t | 0x7F7F7F7Fu);
+		if (!FULL) {                                     /* only bytes of the text */
+			/* rem chunks are left from the start of the stage, the last one padded: bytes of this word inside the text */
+			const int64_t valid = ((int64_t)rem - (int64_t)idx) * 16 - (int64_t)(P.n_chunks * 16 - P.n) - 4 * w;
+			if (valid <= 0) z = 0; else if (valid < 4) z &= (1u << (8 * (uint32_t)valid)) - 1u;
+		}
+		cn += __popc(z);
+	}
+	return cn;
+}
+
 /* the FRONT_CH chunks a thread takes from one stage; FULL = no chunk of the stage is near the end of the text */
 template <int NA, bool MASKED, bool FOLD, bool POLY, bool FULL, bool COUNT, int N3>
 __device__ __forceinline__ void front_chunks(const FrontParams &P, const uint8_t *st, uint32_t tid, uint32_t lane, uint32_t rem, uint32_t *bm, uint16_t *nlb)
@@ -80,22 +101,7 @@ __device__ __forceinline__ void front_chunks(const FrontParams &P, const uint8_t
 		 * the warp's last lane, which costs more issue slots) */
 		uint32_t x4 = *reinterpret_cast<const uint32_t *>(st + idx * 16 + 16);
 		if (COUNT) {
-			/* -n: the delimiter bytes of this chunk (SWAR: 0x80 where a byte equals the delimiter), summed over the warp =
-			 * one 512-byte block of the ordinals pass (aux.cu), which then need not read the text again */
-			const uint32_t xs[4] = { v.x, v.y, v.z, v.w };
-			uint32_t cn = 0;
-#pragma unroll
-			for (int w = 0; w < 4; w++) {
-				const uint32_t t = (xs[w] | P.dfold4) ^ P.delim4;
-				uint32_t z = ~(((t & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | t | 0x7F7F7F7Fu);
-				if (!FULL) {                                     /* only bytes of the text */
-					/* rem chunks are left from the start of the stage, the last one padded: bytes of this word inside the text */
-					const int64_t valid = ((int64_t)rem - (int64_t)idx) * 16 - (int64_t)(P.n_chunks * 16 - P.n) - 4 * w;
-					if (valid <= 0) z = 0; else if (valid < 4) z &= (1u << (8 * (uint32_t)valid)) - 1u;
-				}
-				cn += __popc(z);
-			}
-			const uint32_t blk = __reduce_add_sync(0xffffffffu, cn);
+			const uint32_t blk = __reduce_add_sync(0xffffffffu, chunk_delims<FULL>(P, v, idx, rem));
 			if (lane == 0 && (FULL || idx < rem)) nlb[c * (FRONT_THREADS / 32)] = (uint16_t)blk;
 		}
 		if (FOLD) { v.x |= P.fold; v.y |= P.fold; v.z |= P.fold; v.w |= P.fold; x4 |= P.fold; }
@@ -117,11 +123,85 @@ __device__ __forceinline__ void front_chunks(const FrontParams &P, const uint8_t
 	}
 }
 
+/* ---- the pair plan (DESIGN.md 3.1): k + 2 distinct pieces of len bytes; k errors leave two of them verbatim, and the
+ * second of those starts at most (o_last - o_first) + k <= 16 bytes after the first (the planner checks the bound), so
+ * it starts in the first one's chunk or in the chunk after it.  A chunk is flagged when some piece starts in it and
+ * some other piece starts in it or in its successor. */
+
+/* an IMAD the compiler may not split into a shared multiply and ALU adds (w * scale is the same for every piece) */
+__device__ __forceinline__ uint32_t imad(uint32_t a, uint32_t b, uint32_t c)
+{
+	uint32_t r; asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(c)); return r;
+}
+
+/* bit i = piece i starts in the chunk x[0..3] (x[4]: the word after it).  w * scale + coef[i] = (w - B_i) * 256^(4-len)
+ * vanishes exactly when the low len bytes of window w are piece i: one IMAD per window and piece, half a VIMNMX3 to fold
+ * it; the running minimum starts at 1, so it ends as 0 (present) or 1 */
+template <int NP>
+__device__ __forceinline__ uint32_t piece_bits(const uint32_t (&x)[5], const FrontParams &P)
+{
+	uint32_t acc[NP];
+#pragma unroll
+	for (int i = 0; i < NP; i++) acc[i] = 1u;
+#pragma unroll
+	for (int w = 0; w < 4; w++) {
+		const uint32_t wv[4] = { x[w], __funnelshift_r(x[w], x[w + 1], 8), __funnelshift_r(x[w], x[w + 1], 16), __funnelshift_r(x[w], x[w + 1], 24) };
+#pragma unroll
+		for (int i = 0; i < NP; i++) {
+			acc[i] = __vimin3_u32(acc[i], imad(wv[0], P.scale, P.coef[i]), imad(wv[1], P.scale, P.coef[i]));
+			acc[i] = __vimin3_u32(acc[i], imad(wv[2], P.scale, P.coef[i]), imad(wv[3], P.scale, P.coef[i]));
+		}
+	}
+	uint32_t absent = 0;
+#pragma unroll
+	for (int i = 0; i < NP; i++) absent |= acc[i] << i;
+	return absent ^ ((1u << NP) - 1u);
+}
+
+/* A warp takes FRONT_CH consecutive groups of 32 chunks (bitmap words wid * FRONT_CH + c of the stage), so the successor of
+ * a lane's chunk is the next lane's, or lane 0's of the next group: one SHFL.  The warp's very last chunk (1 in 128) has its
+ * successor in another warp; it is flagged when it holds any piece, which keeps the filter exact. */
+template <int NP, bool FOLD, bool FULL, bool COUNT>
+__device__ __forceinline__ void pair_chunks(const FrontParams &P, const uint8_t *st, uint32_t wid, uint32_t lane, uint32_t rem, uint32_t *bm, uint16_t *nlb)
+{
+	uint32_t pres[FRONT_CH];
+#pragma unroll
+	for (int c = 0; c < FRONT_CH; c++) {
+		const uint32_t idx = (wid * FRONT_CH + c) * 32 + lane;
+		const uint4 v = *reinterpret_cast<const uint4 *>(st + idx * 16);
+		const uint32_t x4 = *reinterpret_cast<const uint32_t *>(st + idx * 16 + 16);
+		if (COUNT) {
+			const uint32_t blk = __reduce_add_sync(0xffffffffu, chunk_delims<FULL>(P, v, idx, rem));
+			if (lane == 0 && (FULL || idx < rem)) nlb[c] = (uint16_t)blk;
+		}
+		const uint32_t f = FOLD ? P.fold : 0u;
+		const uint32_t x[5] = { v.x | f, v.y | f, v.z | f, v.w | f, x4 | f };
+		pres[c] = piece_bits<NP>(x, P);
+	}
+#pragma unroll
+	for (int c = 0; c < FRONT_CH; c++) {
+		const uint32_t idx = (wid * FRONT_CH + c) * 32 + lane;
+		const uint32_t give = (lane == 0 && c + 1 < FRONT_CH) ? pres[c + 1] : pres[c];
+		uint32_t next = __shfl_sync(0xffffffffu, give, (lane + 1) & 31);
+		if (c + 1 == FRONT_CH && lane == 31) next = ~0u;
+		const bool pair = pres[c] != 0 && __popc(pres[c] | next) >= 2;
+		if (FULL) {
+			const uint32_t word = __ballot_sync(0xffffffffu, pair);
+			if (lane == 0) bm[c] = word;
+		} else {
+			/* the last two chunks of the text are always passed on, as in front_chunks */
+			const uint32_t word = __ballot_sync(0xffffffffu, (idx < rem) && (pair || idx + 2 >= rem));
+			if (lane == 0 && idx < rem) bm[c] = word;
+		}
+	}
+}
+
 /* Persistent CTAs.  Thread 0 keeps FRONT_NST bulk copies of 16 KiB (+16 B) in flight into a shared-memory
  * ring, each completing on its own mbarrier; all 256 threads take 4 chunks per stage from shared memory
  * (LDS.128, conflict-free: a warp reads 512 consecutive bytes), test the 16 windows of each chunk and ballot
- * the 32 verdicts of a warp into one bitmap word.  Every text byte crosses HBM->SM once. */
-template <int NA, bool MASKED, bool FOLD, bool POLY, bool COUNT, int N3>
+ * the 32 verdicts of a warp into one bitmap word.  Every text byte crosses HBM->SM once.  NP > 0: the pair plan's test
+ * (pair_chunks) over NP pieces instead of the anchor test. */
+template <int NA, bool MASKED, bool FOLD, bool POLY, bool COUNT, int N3, int NP = 0>
 __global__ void __launch_bounds__(FRONT_THREADS, FRONT_CTAS_PER_SM)
 k_front(const FrontParams P)
 {
@@ -156,24 +236,39 @@ k_front(const FrontParams P)
 		uint32_t *bm = P.bitmap + sg * FRONT_WORDS_PER_STAGE + warp_in_cta;
 		/* full = every chunk of the stage exists and none is among the last two of the text: no per-chunk EOF logic */
 		const bool full = left >= FRONT_STAGE_CHUNKS + 2;
-		uint16_t *nlb = COUNT ? P.nl_blocks + sg * FRONT_WORDS_PER_STAGE + warp_in_cta : nullptr;
-		if (full) front_chunks<NA, MASKED, FOLD, POLY, true, COUNT, N3>(P, st, tid, lane, rem, bm, nlb);
-		else front_chunks<NA, MASKED, FOLD, POLY, false, COUNT, N3>(P, st, tid, lane, rem, bm, nlb);
+		if constexpr (NP > 0) {
+			/* a warp's FRONT_CH words are consecutive here */
+			uint32_t *bmp = P.bitmap + sg * FRONT_WORDS_PER_STAGE + warp_in_cta * FRONT_CH;
+			uint16_t *nlp = COUNT ? P.nl_blocks + sg * FRONT_WORDS_PER_STAGE + warp_in_cta * FRONT_CH : nullptr;
+			if (full) pair_chunks<NP, FOLD, true, COUNT>(P, st, warp_in_cta, lane, rem, bmp, nlp);
+			else pair_chunks<NP, FOLD, false, COUNT>(P, st, warp_in_cta, lane, rem, bmp, nlp);
+		} else {
+			uint16_t *nlb = COUNT ? P.nl_blocks + sg * FRONT_WORDS_PER_STAGE + warp_in_cta : nullptr;
+			if (full) front_chunks<NA, MASKED, FOLD, POLY, true, COUNT, N3>(P, st, tid, lane, rem, bm, nlb);
+			else front_chunks<NA, MASKED, FOLD, POLY, false, COUNT, N3>(P, st, tid, lane, rem, bm, nlb);
+		}
 		__syncthreads();                       /* everyone is done reading this slot */
 		if (tid == 0) issue((uint64_t)it + FRONT_NST);   /* refill it with the stage FRONT_NST iterations ahead */
 	}
 }
 
-template <int NA, bool MASKED, bool FOLD, bool POLY, bool COUNT, int N3>
+template <int NA, bool MASKED, bool FOLD, bool POLY, bool COUNT, int N3, int NP = 0>
 static void launch_front_cnt(const FrontParams &P, unsigned grid, cudaStream_t st)
 {
 	static bool configured[64] = {false};
 	int dev = 0; cudaGetDevice(&dev);
 	if (!configured[dev & 63]) {
-		cudaFuncSetAttribute(k_front<NA, MASKED, FOLD, POLY, COUNT, N3>, cudaFuncAttributeMaxDynamicSharedMemorySize, FRONT_SMEM);
+		cudaFuncSetAttribute(k_front<NA, MASKED, FOLD, POLY, COUNT, N3, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, FRONT_SMEM);
 		configured[dev & 63] = true;
 	}
-	k_front<NA, MASKED, FOLD, POLY, COUNT, N3><<<grid, FRONT_THREADS, FRONT_SMEM, st>>>(P);
+	k_front<NA, MASKED, FOLD, POLY, COUNT, N3, NP><<<grid, FRONT_THREADS, FRONT_SMEM, st>>>(P);
+}
+/* the pair plan over NP pieces */
+template <int NP>
+static void launch_front_pairs(const FrontParams &P, bool fold, unsigned grid, cudaStream_t st)
+{
+	if (P.nl_blocks) { if (fold) launch_front_cnt<0, false, true, true, true, 0, NP>(P, grid, st); else launch_front_cnt<0, false, false, true, true, 0, NP>(P, grid, st); }
+	else             { if (fold) launch_front_cnt<0, false, true, true, false, 0, NP>(P, grid, st); else launch_front_cnt<0, false, false, true, false, 0, NP>(P, grid, st); }
 }
 template <int NA, bool MASKED, bool FOLD, bool POLY, int N3>
 static void launch_front_one(const FrontParams &P, unsigned grid, cudaStream_t st)
@@ -493,6 +588,19 @@ int front_launch(const agb_desc &d, Workspace &W, const void *d_text, uint64_t n
 	}
 	F.one = 1; F.scale = 1; F.s256 = 256;
 	for (int i = d.anchor_len; i < 4; i++) F.scale <<= 8;
+	if (d.pair_plan) {
+		/* the planner made the pieces distinct and at most four (k <= 2) */
+		if (na != d.n_anchors || na < 2 || na > 4 || d.anchor_len < 3) { snprintf(g_err, sizeof g_err, "internal: pair plan with %d pieces", d.n_anchors); return AGB_ERR_ARG; }
+		for (int i = 0; i < na; i++) F.coef[i] = 0u - F.anchor[i] * F.scale;
+		switch (na) {
+		case 2: launch_front_pairs<2>(F, fold, grid, st); break;
+		case 3: launch_front_pairs<3>(F, fold, grid, st); break;
+		default: launch_front_pairs<4>(F, fold, grid, st); break;
+		}
+		g_launches++;
+		CUDA_TRY(cudaGetLastError());
+		return AGB_OK;
+	}
 	bool poly = poly_setup(F.anchor, na, 8 * d.anchor_len, F.coef);
 	if (d.n_anchors3 > 0) {
 		/* mixed plan: the second polynomial over the three-byte anchors; if either guard fails the three-byte anchors join

@@ -853,6 +853,7 @@ int agb_pattern_from_desc(const agb_desc *d, agb_pattern **out, char *err, size_
 		p->d.plan = AGB_PLAN_ALL; p->d.n_anchors = 0; p->d.refine = 0;
 	}
 	if (p->d.n_anchors3 < 0 || p->d.n_anchors3 > 2 || p->d.plan != AGB_PLAN_ANCHORS) p->d.n_anchors3 = 0;
+	p->d.pair_plan = 0;
 	rc = agbi_derive(&p->d, err, errlen);
 	if (rc) { free(p); *out = NULL; return rc; }
 	*out = p;

@@ -296,23 +296,58 @@ static int ordinals_prepare_blocks(const agb_desc &d, Workspace &W, uint64_t n, 
  * and stage 1.5 pays per flagged chunk.  The static plan (pattern.c) takes the first k+1 runs; here, for texts large
  * enough to care, the candidate grams (every literal 4-gram and 3-gram of the pattern) are counted on a 4 MiB sample
  * of the text and the cheapest set is chosen by a small dynamic program: four-byte grams, plus up to two three-byte
- * grams (which cost stage 1 one more operation per window: they only pay when they save enough flags).
+ * grams (which cost stage 1 one more operation per window: they only pay when they save enough flags).  The same sample
+ * also runs the pair plan's rule (k + 2 pieces, a chunk flagged only where two of them meet, DESIGN.md 3.1), which is
+ * taken when it flags clearly fewer chunks than the k+1 plan -- 1.5 % instead of 4.5 % for because each.
  * Works from the Mask[] words alone, so the drop-in layer's descriptors are re-planned too.
  * ---------------------------------------------------------------------------------------------- */
 #define PLAN_MIN_BYTES   (256ull << 20)
 #define PLAN_SAMPLE_BLK  64               /* stretches */
 #define PLAN_BLK_CHUNKS  4096             /* of 64 KiB */
-static int adaptive_plan(const agb_desc &d, Workspace &W, const void *d_text, uint64_t n, cudaStream_t st, agb_desc *out)
+#define PAIR_REACH       16               /* the pair rule sees a second piece up to the end of the next chunk */
+
+/* The pair plan's pieces: k + 2 disjoint literal grams of one length, four bytes if the pattern has room, else three,
+ * pairwise distinct.  k errors damage at most k of them, so two occur verbatim in a match, and the later of those two
+ * starts at most (o_last - o_first) + k bytes after the earlier: with that within PAIR_REACH, the chunk where the
+ * earlier one starts also sees the later one start in it or in the next chunk.  Taken from the left, the first set that
+ * fits.  Returns the number of pieces (0: none). */
+static int pair_pieces(const int *lit, int pat_len, int k, uint32_t fold, uint32_t *val, int *off, int *len_out)
+{
+	const int np = k + 2;
+	if (k < 0 || np > 4) return 0;
+	for (int len = 4; len >= 3; len--)
+		for (int s0 = 0; s0 + np * len <= pat_len; s0++) {
+			int got = 0;
+			for (int p = s0; p + len <= pat_len && got < np; ) {
+				bool ok = true; uint32_t v = 0;
+				for (int t = 0; t < len; t++) { if (lit[p + t] < 0) ok = false; else v |= (uint32_t)(lit[p + t] | (fold & 0x20)) << (8 * t); }
+				if (!ok) { p++; continue; }
+				val[got] = v; off[got] = p; got++; p += len;
+			}
+			if (got < np || off[0] != s0 || off[np - 1] - off[0] + k > PAIR_REACH) continue;
+			bool distinct = true;
+			for (int a = 0; a < np; a++) for (int b = 0; b < a; b++) if (val[a] == val[b]) distinct = false;
+			if (!distinct) continue;
+			*len_out = len;
+			return np;
+		}
+	return 0;
+}
+
+static int adaptive_plan(const agb_desc &d, Workspace &W, const void *d_text, uint64_t n, bool count_delims, cudaStream_t st, agb_desc *out)
 {
 	*out = d;
 	if (!d.adaptive || !front_usable(d) || !d.refine || d.n_anchors3 || n < PLAN_MIN_BYTES || d.pat_len < 4 || d.pat_len > 60) return AGB_OK;
 	const int need = d.k + 1;
 	if (need > 9) return AGB_OK;
+	const char *pp = getenv("AGB_PLAN_PAIRS");          /* unset: the pair plan when the sample favours it; 0: never; 1: whenever it exists */
+	const int pairs_env = (pp && *pp) ? atoi(pp) : -1;
 	uint64_t key = 1469598103934665603ull;
 	{
 		const unsigned char *b = (const unsigned char *)&d;
 		for (size_t i = 0; i < sizeof d; i++) { key ^= b[i]; key *= 1099511628211ull; }
 		key ^= (uint64_t)(uintptr_t)d_text; key *= 1099511628211ull; key ^= n; key *= 1099511628211ull;
+		key ^= (uint64_t)(pairs_env + 2) * 2 + (count_delims ? 1 : 0); key *= 1099511628211ull;
 	}
 	if (W.plan_valid && W.plan_key == key) { *out = W.plan_desc; return AGB_OK; }
 	/* literal bytes of the pattern proper, from the masks */
@@ -336,19 +371,28 @@ static int adaptive_plan(const agb_desc &d, Workspace &W, const void *d_text, ui
 			if (!ok) continue;
 			g[ng].s = s; g[ng].len = len; g[ng].v = v; g[ng].m = len == 4 ? 0xFFFFFFFFu : 0x00FFFFFFu; g[ng].cost = 0; ng++;
 		}
-	if (ng < need) return AGB_OK;
+	/* the pair plan's pieces are sampled along with the grams (behind them) */
+	uint32_t pv[4]; int poff[4], plen = 0;
+	const int n_pair = pairs_env != 0 ? pair_pieces(lit, d.pat_len, d.k, fold, pv, poff, &plen) : 0;
+	if (ng < need && !n_pair) return AGB_OK;
 	if (!W.d_gram) { CUDA_TRY(cudaMalloc(&W.d_gram, 3 * 128 * sizeof(uint32_t))); CUDA_TRY(cudaMallocHost(&W.h_gram, 3 * 128 * sizeof(uint32_t))); }
-	for (int i = 0; i < 128; i++) { W.h_gram[i] = i < ng ? g[i].v : 0; W.h_gram[128 + i] = i < ng ? g[i].m : 0; W.h_gram[256 + i] = 0; }
+	for (int i = 0; i < 128; i++) {
+		const bool gi = i < ng, pi = i >= ng && i < ng + n_pair;
+		W.h_gram[i] = gi ? g[i].v : pi ? pv[i - ng] : 0;
+		W.h_gram[128 + i] = gi ? g[i].m : pi ? (plen == 4 ? 0xFFFFFFFFu : 0x00FFFFFFu) : 0;
+		W.h_gram[256 + i] = 0;
+	}
 	CUDA_TRY(cudaMemcpyAsync(W.d_gram, W.h_gram, 3 * 128 * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
 	const uint64_t n_chunks = (n + 15) / 16;
 	const uint64_t threads = (uint64_t)PLAN_SAMPLE_BLK * PLAN_BLK_CHUNKS;
 	k_gram_sample<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>((const uint8_t *)d_text, n_chunks, PLAN_SAMPLE_BLK, PLAN_BLK_CHUNKS,
-	                                                                 ng, W.d_gram, W.d_gram + 128, fold, W.d_gram + 256);
+	                                                                 ng + n_pair, W.d_gram, W.d_gram + 128, fold, W.d_gram + 256, ng, n_pair);
 	g_launches++;
 	CUDA_TRY(cudaGetLastError());
 	CUDA_TRY(cudaMemcpyAsync(W.h_gram + 256, W.d_gram + 256, 128 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
 	CUDA_TRY(cudaStreamSynchronize(st));
 	for (int i = 0; i < ng; i++) g[i].cost = (double)W.h_gram[256 + i] / (double)threads;
+	const double pair_rate = (double)W.h_gram[256 + 127] / (double)threads;
 	/* dynamic program over the pattern positions: f[p][j][t] = least total rate of j disjoint grams inside [0, p), t of them
 	 * three bytes long */
 	/* what a three-byte group costs, in units of flag rate: on the benchmark pattern (beca|se e|ach flags 2.4 % of the
@@ -379,39 +423,62 @@ static int adaptive_plan(const agb_desc &d, Workspace &W, const void *d_text, ui
 	}
 	double cur = 0;                                     /* the static plan's rate, from the same sample where it can be read off */
 	for (int a = 0; a < d.n_anchors; a++) { double r = 1.0; for (int i = 0; i < ng; i++) if (g[i].len == d.anchor_len && g[i].s == d.anchor_off[a]) r = g[i].cost; cur += r; }
-	if (best_t < 0 || !(best < 0.85 * cur)) { W.plan_key = key; W.plan_valid = true; W.plan_desc = d; return AGB_OK; }
-	agb_desc nd = d;
-	nd.n_anchors = 0; nd.n_anchors3 = 0; nd.anchor_len = 4; nd.anchor_mask = 0xFFFFFFFFu; nd.anchor_fold = fold;
-	{
-		int p = d.pat_len, j = need, t = best_t;
-		while (p > 0 && j >= 0) {
-			const int fr = from[p][j][t];
-			if (fr == -1) { p--; continue; }
-			if (fr < 0) break;
-			if (g[fr].len == 4) { nd.anchor[nd.n_anchors] = g[fr].v; nd.anchor_off[nd.n_anchors] = g[fr].s; nd.n_anchors++; }
-			else { nd.anchor3[nd.n_anchors3] = g[fr].v; nd.anchor3_off[nd.n_anchors3] = g[fr].s; nd.n_anchors3++; }
-			p -= g[fr].len; j--; t -= (g[fr].len == 3);
+	/* the k+1 plan: the static one unless the sample says a set of grams flags clearly fewer chunks */
+	agb_desc plan = d;
+	double rate = cur;
+	if (best_t >= 0 && best < 0.85 * cur) {
+		agb_desc nd = d;
+		nd.n_anchors = 0; nd.n_anchors3 = 0; nd.anchor_len = 4; nd.anchor_mask = 0xFFFFFFFFu; nd.anchor_fold = fold;
+		{
+			int p = d.pat_len, j = need, t = best_t;
+			while (p > 0 && j >= 0) {
+				const int fr = from[p][j][t];
+				if (fr == -1) { p--; continue; }
+				if (fr < 0) break;
+				if (g[fr].len == 4) { nd.anchor[nd.n_anchors] = g[fr].v; nd.anchor_off[nd.n_anchors] = g[fr].s; nd.n_anchors++; }
+				else { nd.anchor3[nd.n_anchors3] = g[fr].v; nd.anchor3_off[nd.n_anchors3] = g[fr].s; nd.n_anchors3++; }
+				p -= g[fr].len; j--; t -= (g[fr].len == 3);
+			}
+		}
+		/* the kernels want their polynomials: both groups must pass the false-positive guard, and the anchors must be
+		 * pairwise distinct (stage 1.5 tells them apart by their bytes) */
+		bool ok = nd.n_anchors + nd.n_anchors3 == need && nd.n_anchors >= 1;
+		uint32_t tmp[AGB_MAXANCHOR];
+		if (ok) ok = poly_setup(nd.anchor, nd.n_anchors, 32, tmp);
+		if (ok && nd.n_anchors3) ok = poly_setup(nd.anchor3, nd.n_anchors3, 24, tmp);
+		for (int a = 0; a < nd.n_anchors && ok; a++) {
+			for (int b = 0; b < a; b++) if (nd.anchor[a] == nd.anchor[b]) ok = false;
+			for (int b = 0; b < nd.n_anchors3; b++) if ((nd.anchor[a] & 0x00FFFFFFu) == nd.anchor3[b]) ok = false;
+		}
+		for (int a = 0; a < nd.n_anchors3 && ok; a++) for (int b = 0; b < a; b++) if (nd.anchor3[a] == nd.anchor3[b]) ok = false;
+		if (ok) { plan = nd; rate = best; }
+		if (getenv("AGB_DEBUG_PLAN")) {
+			fprintf(stderr, "agb plan: static rate %.4f -> %s rate %.4f:", cur, ok ? "chosen" : "rejected", best);
+			for (int a = 0; a < nd.n_anchors; a++) fprintf(stderr, " [%.4s]@%d", (const char *)&nd.anchor[a], nd.anchor_off[a]);
+			for (int a = 0; a < nd.n_anchors3; a++) fprintf(stderr, " [%.3s]@%d", (const char *)&nd.anchor3[a], nd.anchor3_off[a]);
+			fprintf(stderr, "\n");
 		}
 	}
-	/* the kernels want their polynomials: both groups must pass the false-positive guard, and the anchors must be
-	 * pairwise distinct (stage 1.5 tells them apart by their bytes) */
-	bool ok = nd.n_anchors + nd.n_anchors3 == need && nd.n_anchors >= 1;
-	uint32_t tmp[AGB_MAXANCHOR];
-	if (ok) ok = poly_setup(nd.anchor, nd.n_anchors, 32, tmp);
-	if (ok && nd.n_anchors3) ok = poly_setup(nd.anchor3, nd.n_anchors3, 24, tmp);
-	for (int a = 0; a < nd.n_anchors && ok; a++) {
-		for (int b = 0; b < a; b++) if (nd.anchor[a] == nd.anchor[b]) ok = false;
-		for (int b = 0; b < nd.n_anchors3; b++) if ((nd.anchor[a] & 0x00FFFFFFu) == nd.anchor3[b]) ok = false;
+	/* the pair plan, by the same margin against the k+1 plan's rate (a sum over its grams: an upper bound).  Not when
+	 * stage 1 also counts the delimiters (-n): its 24 more ALU operations per chunk on top of the pair test make stage 1
+	 * cost about what stage 1.5 saves (on H100 the -n headline took 17.75 ms against 17.70 ms) */
+	if (n_pair) {
+		const bool take = pairs_env == 1 || (!count_delims && pair_rate < 0.85 * rate);
+		if (take) {
+			agb_desc pd = d;
+			pd.pair_plan = 1; pd.n_anchors = n_pair; pd.n_anchors3 = 0; pd.anchor_len = plen;
+			pd.anchor_mask = plen == 4 ? 0xFFFFFFFFu : 0x00FFFFFFu; pd.anchor_fold = fold;
+			for (int i = 0; i < n_pair; i++) { pd.anchor[i] = pv[i]; pd.anchor_off[i] = poff[i]; }
+			plan = pd;
+		}
+		if (getenv("AGB_DEBUG_PLAN")) {
+			fprintf(stderr, "agb plan: k+1 rate %.4f, pair rate %.4f -> pair plan %s:", rate, pair_rate, take ? "chosen" : "not chosen");
+			for (int i = 0; i < n_pair; i++) fprintf(stderr, " [%.*s]@%d", plen, (const char *)&pv[i], poff[i]);
+			fprintf(stderr, "\n");
+		}
 	}
-	for (int a = 0; a < nd.n_anchors3 && ok; a++) for (int b = 0; b < a; b++) if (nd.anchor3[a] == nd.anchor3[b]) ok = false;
-	W.plan_key = key; W.plan_valid = true; W.plan_desc = ok ? nd : d;
-	*out = W.plan_desc;
-	if (getenv("AGB_DEBUG_PLAN")) {
-		fprintf(stderr, "agb plan: static rate %.4f -> %s rate %.4f:", cur, ok ? "chosen" : "rejected", best);
-		for (int a = 0; a < nd.n_anchors; a++) fprintf(stderr, " [%.4s]@%d", (const char *)&nd.anchor[a], nd.anchor_off[a]);
-		for (int a = 0; a < nd.n_anchors3; a++) fprintf(stderr, " [%.3s]@%d", (const char *)&nd.anchor3[a], nd.anchor3_off[a]);
-		fprintf(stderr, "\n");
-	}
+	W.plan_key = key; W.plan_valid = true; W.plan_desc = plan;
+	*out = plan;
 	return AGB_OK;
 }
 
@@ -489,7 +556,7 @@ int scan_device_impl(const agb_desc &d_in, const void *d_text, uint64_t n, int w
 	Workspace &W = g_ws[dev];
 	int rc = ws_prepare(W, n); if (rc) return rc;
 	agb_desc planned;
-	rc = adaptive_plan(d_in, W, d_text, n, st, &planned); if (rc) return rc;
+	rc = adaptive_plan(d_in, W, d_text, n, (want & AGB_WANT_ORDINALS) && d_in.L == 1, st, &planned); if (rc) return rc;
 	const agb_desc &d = planned;
 	if (want == AGB_WANT_COUNT && !sh && n >= (1u << 20) && exact_count_usable(d)) {
 		/* `agrep -c the`: an exact literal no longer than its anchor needs no automaton (front.cu, exact_count_launch) */

@@ -214,7 +214,8 @@ int  launch_regex(const agb_desc &d, const RecParams &P, unsigned grid, cudaStre
 size_t regex_tables(const agb_desc &d, const agb_regex &rx, uint64_t *out);
 /* aux.cu */
 __global__ void k_gram_sample(const uint8_t *text, uint64_t n_chunks, uint32_t nblk, uint32_t blk_chunks,
-                              int ngram, const uint32_t *gram, const uint32_t *gmask, uint32_t fold, unsigned int *counts);
+                              int ngram, const uint32_t *gram, const uint32_t *gmask, uint32_t fold, unsigned int *counts,
+                              int pair_first, int n_pair);
 __global__ void k_compact_count(const uint32_t *bitmap, uint64_t n_words, uint32_t *block_counts, unsigned long long *totals);
 __global__ void k_compact_write(const uint32_t *bitmap, uint64_t n_words, const uint64_t *block_offsets, uint64_t *cand, uint64_t cand_cap);
 __global__ void k_scan_tiles(const uint32_t *counts, uint64_t *offsets, uint64_t n_tiles, unsigned long long *total);

@@ -100,7 +100,10 @@ typedef struct agb_desc {
 	 * delimiter included, maskgen.c:52-58, 259-266), else 0: away from the automaton a delimiter byte c is recognised by
 	 * (c | delim_fold[p]) == (delim[p] | delim_fold[p]); filled by agb_compile / agb_pattern_from_desc from mask[] */
 	uint8_t  delim_fold[2 * AGB_MAXDELIM + 2];
-	uint8_t  pad_[2];
+	/* 1: the anchors are the k + 2 equal-length pieces of the pair plan -- stage 1 flags a chunk only where one piece starts
+	 * and another one starts in it or in the chunk after it (set by the device scan's planner only; 0 from every caller) */
+	uint8_t  pair_plan;
+	uint8_t  pad_[1];
 } agb_desc;
 
 typedef struct agb_pattern agb_pattern;       /* opaque: agb_desc + bookkeeping              */
