@@ -342,14 +342,28 @@ static int adaptive_plan(const agb_desc &d, Workspace &W, const void *d_text, ui
 	if (need > 9) return AGB_OK;
 	const char *pp = getenv("AGB_PLAN_PAIRS");          /* unset: the pair plan when the sample favours it; 0: never; 1: whenever it exists */
 	const int pairs_env = (pp && *pp) ? atoi(pp) : -1;
+	/* what a three-byte group costs, in units of flag rate (the dynamic program below): part of the key, so that a
+	 * change of AGB_PLAN_MIXED between two scans of one text plans afresh */
+	const char *mp = getenv("AGB_PLAN_MIXED");           /* (tests force mixed plans with AGB_PLAN_MIXED=0) */
+	const double MIXED = mp ? atof(mp) : 0.03;
 	uint64_t key = 1469598103934665603ull;
 	{
 		const unsigned char *b = (const unsigned char *)&d;
 		for (size_t i = 0; i < sizeof d; i++) { key ^= b[i]; key *= 1099511628211ull; }
 		key ^= (uint64_t)(uintptr_t)d_text; key *= 1099511628211ull; key ^= n; key *= 1099511628211ull;
 		key ^= (uint64_t)(pairs_env + 2) * 2 + (count_delims ? 1 : 0); key *= 1099511628211ull;
+		uint64_t mbits; memcpy(&mbits, &MIXED, sizeof mbits);
+		key ^= mbits; key *= 1099511628211ull;
 	}
-	if (W.plan_valid && W.plan_key == key) { *out = W.plan_desc; return AGB_OK; }
+	if (W.plan_valid && W.plan_key == key) {
+		*out = W.plan_desc;
+		if (getenv("AGB_DEBUG_PLAN") && out->pair_plan) {            /* a scan that reuses the plan says so too */
+			fprintf(stderr, "agb plan: cached -> pair plan chosen:");
+			for (int i = 0; i < out->n_anchors; i++) fprintf(stderr, " [%.*s]@%d", out->anchor_len, (const char *)&out->anchor[i], out->anchor_off[i]);
+			fprintf(stderr, "\n");
+		}
+		return AGB_OK;
+	}
 	/* literal bytes of the pattern proper, from the masks */
 	int lit[64]; bool pair_any = false;
 	for (int j = 0; j < d.pat_len; j++) {
@@ -398,9 +412,8 @@ static int adaptive_plan(const agb_desc &d, Workspace &W, const void *d_text, ui
 	/* what a three-byte group costs, in units of flag rate: on the benchmark pattern (beca|se e|ach flags 2.4 % of the
 	 * chunks instead of 4.5 %) stage 1 pays for a second polynomial and one VIMNMX3 per window instead of half of one,
 	 * and stage 1.5 does not get cheaper in proportion -- a mixed plan only pays when the four-byte grams of a piece
-	 * are really common */
-	const char *mp = getenv("AGB_PLAN_MIXED");           /* (tests force mixed plans with AGB_PLAN_MIXED=0) */
-	const double INF = 1e30, MIXED = mp ? atof(mp) : 0.03;
+	 * are really common (MIXED, above) */
+	const double INF = 1e30;
 	static double f[66][10][3]; static int from[66][10][3];   /* gram taken to get here, -1: position skipped */
 	for (int p = 0; p <= d.pat_len; p++) for (int j = 0; j <= need; j++) for (int t = 0; t < 3; t++) { f[p][j][t] = INF; from[p][j][t] = -2; }
 	f[0][0][0] = 0;

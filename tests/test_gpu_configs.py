@@ -88,8 +88,8 @@ def test_anchor_planner_plans_agree(monkeypatch):
             monkeypatch.setenv("AGB_PLAN_MIXED", env)
         for pat, kw in pats:
             rec = torch.zeros((cap, 4), dtype=torch.int64, device="cuda")
-            # a fresh text pointer per setting would defeat nothing: the plan is cached per (descriptor, text); change k's
-            # sibling field instead -- a new Pattern object has the same descriptor, so shift the text by one page
+            # each setting scans the text shifted by one page more: three overlapping texts, compared below where they
+            # overlap (the plan cache's key covers AGB_PLAN_MIXED, so the shift is not what makes each setting re-plan)
             off = {None: 0, "0": 4096, "10": 8192}[env]
             r = ag.Pattern(pat, **kw).scan_device(t.data_ptr() + off, n - 16384, d_records=rec.data_ptr(), capacity=cap)
             lists.append((env, pat, off, int(r.n_matched), (rec[:r.n_records, :2] + off).cpu()))

@@ -1,7 +1,9 @@
 """The pair plan on the device (stage 1 flags a chunk only where two different pieces of the pattern meet; DESIGN.md 3.1),
 forced on and forced off with AGB_PLAN_PAIRS: both give the checker's counts, records, levels and ordinals.  The planner
-only re-plans texts of 256 MiB and more, so the texts here are that large; planted matches with 0..k edits put their two
-surviving pieces across a chunk boundary, a warp's last chunk (2 KiB), a 16 KiB stage boundary and the end of the text."""
+only re-plans texts of 256 MiB and more that are scanned in device memory (scan_device, the shard-local scan, and each
+window of 256 MiB or more of a windowed host scan; the whole-text host scan is not planned), so the texts here are that
+large; planted matches with 0..k edits put their two surviving pieces across a chunk boundary, a warp's last chunk
+(2 KiB), a 16 KiB stage boundary and the end of the text.  tests/test_gpu_plans_large.py covers the other pair plans."""
 import ctypes as C
 import os, random
 import pytest
@@ -97,6 +99,8 @@ def test_forced_on_and_off_match_the_checker(text, dev, pairs, capfd, nocase):
 
 
 def test_count_and_host_entry_points(text, dev, pairs):
+    """the count-only device scan and the windowed host scan (its first window, 256 MiB plus halos, is planned) under
+    both settings; the whole-text host scan is not planned, so there both settings run the static plan"""
     pat = ag.Pattern(PATTERN, k=K)
     cnt, expect = _oracle.scan(_oracle.compile(PATTERN, k=K, linenum=1), text, cap=1 << 20)
     for v in (0, 1):
