@@ -22,6 +22,8 @@
 #include <unistd.h>
 #include <fcntl.h>
 #include <sys/stat.h>
+#include <functional>
+#include <memory>
 #include <mutex>
 #include <thread>
 
@@ -32,27 +34,25 @@ std::atomic<uint64_t> g_launches{0};
 extern "C" const char *agb_last_error(void) { return g_err; }
 extern "C" const char *agb_version(void) { return "agrep-b200 0.1 (sm_90a)"; }
 extern "C" uint64_t agb_kernel_launches(void) { return g_launches.load(); }
-static void win_release(int dev);
+static void host_release(int dev);
 /* frees the per-device scratch of this process (bitmaps, candidate lists, pinned rings, streams, events); the next
  * scan allocates again */
 extern "C" void agb_shutdown(void)
 {
 	int cur = 0; cudaGetDevice(&cur);
 	for (int dev = 0; dev < 64; dev++) {
-		win_release(dev);
+		host_release(dev);
 		std::lock_guard<std::mutex> lk(g_ws_mu[dev]);
 		Workspace &W = g_ws[dev];
-		if (!W.totals && !W.bitmap && !W.h2d_text) continue;
+		if (!W.totals && !W.bitmap) continue;
 		if (cudaSetDevice(dev) != cudaSuccess) { cudaGetLastError(); continue; }
 		cudaDeviceSynchronize();
 		cudaFree(W.bitmap); cudaFree(W.bitmap2); cudaFree(W.range_counts); cudaFree(W.range_offsets);
 		cudaFree(W.tile_counts); cudaFree(W.tile_offsets); cudaFree(W.cand); cudaFree(W.cand_counts); cudaFree(W.cand_offsets);
 		cudaFree(W.cand_first); cudaFree(W.scan_sums); cudaFree(W.scan_offs); cudaFree(W.ord_blocks); cudaFree(W.totals);
-		cudaFreeHost(W.h_totals); cudaFree(W.d_desc); cudaFree(W.h2d_text); cudaFree(W.h2d_rec); cudaFree(W.d_gram); cudaFreeHost(W.h_gram);
+		cudaFreeHost(W.h_totals); cudaFree(W.d_desc); cudaFree(W.d_gram); cudaFreeHost(W.h_gram);
 		cudaFree(W.d_regex);
 		if (W.e0) cudaEventDestroy(W.e0); if (W.e1) cudaEventDestroy(W.e1); if (W.e2) cudaEventDestroy(W.e2);
-		for (int i = 0; i < STAGE_BUFS; i++) { if (W.ev_copy[i]) cudaEventDestroy(W.ev_copy[i]); if (W.stage[i]) cudaFreeHost(W.stage[i]); }
-		if (W.s_copy) cudaStreamDestroy(W.s_copy); if (W.s_comp) cudaStreamDestroy(W.s_comp);
 		W = Workspace();
 	}
 	cudaSetDevice(cur);
@@ -608,54 +608,12 @@ extern "C" int agb_scan_device(const agb_pattern *p, const void *d_text, uint64_
 	return scan_device_impl(p->d, d_text, n, want, -1, d_records, capacity, (cudaStream_t)stream, res, nullptr, agb_pattern_regex(p));
 }
 
-static void par_memcpy(uint8_t *dst, const uint8_t *src, size_t len)
-{
-	const int T = 4; const size_t part = ((len + T - 1) / T + 4095) & ~(size_t)4095;
-	std::thread th[T]; int used = 0;
-	for (int t = 0; t < T; t++) {
-		size_t a = (size_t)t * part; if (a >= len) break;
-		size_t l = std::min(part, len - a);
-		th[used++] = std::thread([=] { memcpy(dst + a, src + a, l); });
-	}
-	for (int t = 0; t < used; t++) th[t].join();
-}
-
-/* Host text -> HBM -> scan: the replacement of the fill_buf()/read(2) loop (bitap.c:143,450-477).  The text is
- * moved in 64 MiB slices on a copy stream -- straight from the caller's memory when it is page-locked; through a
- * pinned ring filled by 4 host threads when it is pageable; pread(2) by 4 threads straight into the pinned ring when the
- * source is a regular file -- while stage 1 runs on the slice that arrived before (its last chunk looks 4
- * bytes into the next one), so the scan hides behind PCIe; stages 1.5 and 2 run once over the whole bitmap. */
-struct SliceSource {
-	const uint8_t *mem;      /* host memory source, or NULL */
-	bool pinned;             /* mem is page-locked: copy from it directly */
-	int fd;                  /* file descriptor source when mem == NULL (a regular file) */
-	off_t fd_off = 0;        /* where the text starts in it */
-};
-
-/* a slice of a regular file into the pinned ring: 4 host threads pread(2) a quarter each (one thread's read(2) from the page
- * cache is a third of what PCIe takes).  direct: fd was opened with O_DIRECT -- whole 4 KiB blocks are asked for (the ring's
- * buffers are page aligned and a multiple of 4 KiB long; the file's last block comes back short) */
-static bool par_pread(int fd, off_t at, uint8_t *dst, size_t len, bool direct)
-{
-	const int T = 4; const size_t part = ((len + T - 1) / T + 4095) & ~(size_t)4095;
-	std::thread th[T]; int used = 0; std::atomic<int> bad{0};
-	for (int t = 0; t < T; t++) {
-		size_t a = (size_t)t * part; if (a >= len) break;
-		size_t l = std::min(part, len - a);
-		th[used++] = std::thread([=, &bad] {
-			size_t got = 0;
-			while (got < l) {
-				const size_t ask = direct ? ((l - got + 4095) & ~(size_t)4095) : l - got;
-				ssize_t r = pread(fd, dst + a + got, ask, at + (off_t)(a + got));
-				if (r <= 0 || (direct && (size_t)r < l - got && ((size_t)r & 4095))) { bad = 1; return; }
-				got += std::min((size_t)r, l - got);
-			}
-		});
-	}
-	for (int t = 0; t < used; t++) th[t].join();
-	return bad == 0;
-}
-
+/* Host text -> HBM -> scan: the replacement of the fill_buf()/read(2) loop (bitap.c:143,450-477).  The text is moved in
+ * 64 MiB slices on a copy stream -- straight from the caller's memory when it is page-locked; through a pinned ring filled
+ * by 4 host threads when it is pageable; pread(2) by 4 threads into the ring from a regular file -- while stage 1 runs on
+ * the slice that arrived before (its last chunk looks 4 bytes into the next one), so the scan hides behind PCIe; stages 1.5
+ * and 2 run once over the whole bitmap.  The whole-text, windowed and resident-text uploads share this one loop (upload),
+ * one pinned ring and one pair of streams per device (HostPath). */
 /* AGB_ODIRECT=1: read regular files past the page cache (a second descriptor on the same file, through /proc/self/fd);
  * -1 when not asked for, when the text does not start on a block boundary, or when the file system refuses */
 static int open_direct(int fd, off_t fd_off)
@@ -665,15 +623,143 @@ static int open_direct(int fd, off_t fd_off)
 	char path[64]; snprintf(path, sizeof path, "/proc/self/fd/%d", fd);
 	return open(path, O_RDONLY | O_DIRECT);
 }
-struct FdGuard { int fd = -1; ~FdGuard() { if (fd >= 0) close(fd); } };
-/* one slice of the file into dst; falls back to the caller's own descriptor for good if the direct one fails */
-static bool read_slice(const SliceSource &src, int *dfd, uint64_t off, uint8_t *dst, size_t len)
-{
-	if (*dfd >= 0) {
-		if (par_pread(*dfd, src.fd_off + (off_t)off, dst, len, true)) return true;
-		close(*dfd); *dfd = -1;
+
+/* the n bytes of text a host path moves: host memory, or a regular file from fd_off on (fd_source) */
+struct SliceSource {
+	const uint8_t *mem = nullptr;  /* host memory source, or NULL */
+	bool pinned = false;           /* mem is page-locked: copy from it directly */
+	int fd = -1;                   /* file descriptor source when mem == NULL (a regular file) */
+	off_t fd_off = 0;              /* where the text starts in it (-1: lseek failed, and n is 0) */
+	int dfd = -1;                  /* the same file opened with O_DIRECT, or -1; closed for good when a read through it fails */
+	uint64_t n = 0;
+	SliceSource(const void *h_text = nullptr, uint64_t len = 0) : mem((const uint8_t *)h_text), n(len)
+	{
+		cudaPointerAttributes attr; memset(&attr, 0, sizeof attr);
+		pinned = len && cudaPointerGetAttributes(&attr, h_text) == cudaSuccess && attr.type == cudaMemoryTypeHost;
+		cudaGetLastError();
 	}
-	return par_pread(src.fd, src.fd_off + (off_t)off, dst, len, false);
+	SliceSource(const SliceSource &) = delete;
+	SliceSource &operator=(const SliceSource &) = delete;
+	~SliceSource() { if (dfd >= 0) close(dfd); }
+};
+
+/* a regular file from the descriptor's offset to its end (false: not a regular file) */
+static bool fd_source(int fd, SliceSource &src)
+{
+	struct stat sb;
+	if (fstat(fd, &sb) != 0 || !S_ISREG(sb.st_mode)) return false;
+	src.fd = fd; src.fd_off = lseek(fd, 0, SEEK_CUR);
+	src.n = (src.fd_off >= 0 && sb.st_size > src.fd_off) ? (uint64_t)(sb.st_size - src.fd_off) : 0;
+	src.dfd = open_direct(fd, src.fd_off);
+	return true;
+}
+
+/* bytes [off, off + len) of a pageable or file source into the ring buffer dst: 4 host threads memcpy or pread(2) a quarter
+ * each (one thread's memcpy, or read(2) from the page cache, is a third of what PCIe takes; under 1 MiB of memory one thread
+ * does).  Through the O_DIRECT descriptor whole 4 KiB blocks are asked for (the ring's buffers are page aligned and a multiple
+ * of 4 KiB long; the file's last block comes back short); when that fails, the caller's own descriptor is used for good. */
+static bool fill_slice(SliceSource &src, uint64_t off, uint8_t *dst, size_t len)
+{
+	if (src.mem && len < (1u << 20)) { memcpy(dst, src.mem + off, len); return true; }
+	for (;;) {
+		const bool direct = !src.mem && src.dfd >= 0;
+		const int fd = direct ? src.dfd : src.fd, T = 4;
+		const size_t part = ((len + T - 1) / T + 4095) & ~(size_t)4095;
+		std::thread th[T]; int used = 0; std::atomic<int> bad{0};
+		for (int t = 0; t < T; t++) {
+			const size_t a = (size_t)t * part; if (a >= len) break;
+			const size_t l = std::min(part, len - a);
+			const uint8_t *mem = src.mem ? src.mem + off + a : nullptr;
+			const off_t at = src.fd_off + (off_t)(off + a);
+			th[used++] = std::thread([=, &bad] {
+				if (mem) { memcpy(dst + a, mem, l); return; }
+				for (size_t got = 0; got < l; ) {
+					const size_t ask = direct ? ((l - got + 4095) & ~(size_t)4095) : l - got;
+					ssize_t r = pread(fd, dst + a + got, ask, at + (off_t)got);
+					if (r <= 0 || (direct && (size_t)r < l - got && ((size_t)r & 4095))) { bad = 1; return; }
+					got += std::min((size_t)r, l - got);
+				}
+			});
+		}
+		for (int t = 0; t < used; t++) th[t].join();
+		if (!bad || !direct) return !bad;
+		close(src.dfd); src.dfd = -1;
+	}
+}
+
+/* Per device, kept until agb_shutdown(): the copy and compute streams, the pinned ring and its events, the whole text of
+ * agb_scan_host / agb_scan_fd and the device list behind records delivered to host memory.  A call holds g_host_mu[dev]
+ * throughout.  Lock order: g_host_mu[dev] first, then g_ws_mu[dev] (in scan_device_impl and its kin), never the reverse. */
+struct HostPath {
+	cudaStream_t s_copy = nullptr, s_comp = nullptr;
+	cudaEvent_t ev[STAGE_BUFS] = {nullptr, nullptr, nullptr};
+	uint8_t *ring[STAGE_BUFS] = {nullptr, nullptr, nullptr};
+	uint8_t *text = nullptr; size_t text_cap = 0;          /* (capacities in bytes) */
+	agb_record *rec = nullptr; size_t rec_cap = 0;
+};
+static HostPath g_host[64];
+static std::mutex g_host_mu[64];
+
+/* the streams and events; the ring only when the source goes through it */
+static int host_ensure(HostPath &H, const SliceSource &src)
+{
+	if (!H.s_copy) CUDA_TRY(cudaStreamCreateWithFlags(&H.s_copy, cudaStreamNonBlocking));
+	if (!H.s_comp) CUDA_TRY(cudaStreamCreateWithFlags(&H.s_comp, cudaStreamNonBlocking));
+	for (int i = 0; i < STAGE_BUFS; i++) if (!H.ev[i]) CUDA_TRY(cudaEventCreateWithFlags(&H.ev[i], cudaEventDisableTiming));
+	if (src.n && !src.pinned) for (int i = 0; i < STAGE_BUFS; i++) if (!H.ring[i]) CUDA_TRY(cudaMallocHost(&H.ring[i], H2D_SLICE));
+	return AGB_OK;
+}
+
+static void host_release(int dev)
+{
+	std::lock_guard<std::mutex> lk(g_host_mu[dev]);
+	HostPath &H = g_host[dev];
+	if (!H.s_copy && !H.text && !H.rec) return;              /* (the events and the ring are made after s_copy) */
+	if (cudaSetDevice(dev) != cudaSuccess) { cudaGetLastError(); return; }
+	cudaDeviceSynchronize();
+	for (int i = 0; i < STAGE_BUFS; i++) { if (H.ev[i]) cudaEventDestroy(H.ev[i]); cudaFreeHost(H.ring[i]); }
+	if (H.s_copy) cudaStreamDestroy(H.s_copy); if (H.s_comp) cudaStreamDestroy(H.s_comp);
+	cudaFree(H.text); cudaFree(H.rec);
+	H = HostPath();
+}
+
+/* *p grown to `bytes` of device memory (what it held is not kept); a failed allocation leaves it NULL, the error cleared */
+template <class T> static cudaError_t dev_reserve(T **p, size_t *cap, size_t bytes)
+{
+	if (bytes <= *cap) return cudaSuccess;
+	cudaFree(*p); *p = nullptr; *cap = 0;
+	const cudaError_t e = cudaMalloc(p, bytes);
+	if (e != cudaSuccess) { *p = nullptr; cudaGetLastError(); return e; }
+	*cap = bytes;
+	return cudaSuccess;
+}
+
+/* bytes [lo, hi) of the source to dst on s_copy in H2D_SLICE pieces, straight from page-locked memory or through the ring,
+ * after `slack` zero bytes at dst + (hi - lo) (stage 1 reads 16 bytes past its last chunk): every slice's event comes after
+ * the zeroing.  after(i, ev) runs once slice i's copy is enqueued and ev recorded behind it.  Does not wait for the copies,
+ * except on an error: then s_copy is drained first, so that no copy out of the ring or into dst is left in flight. */
+static int upload(HostPath &H, SliceSource &src, uint64_t lo, uint64_t hi, uint8_t *dst, uint64_t slack,
+                  const std::function<int(uint64_t, cudaEvent_t)> &after = nullptr)
+{
+	struct Drain { cudaStream_t s; bool on = true; ~Drain() { if (on) cudaStreamSynchronize(s); } } drain{H.s_copy};
+	CUDA_TRY(cudaMemsetAsync(dst + (hi - lo), 0, slack, H.s_copy));
+	for (uint64_t i = 0, off = lo; off < hi; i++, off += H2D_SLICE) {
+		const uint64_t len = std::min<uint64_t>(H2D_SLICE, hi - off);
+		const int sb = (int)(i % STAGE_BUFS);
+		if (src.pinned) CUDA_TRY(cudaMemcpyAsync(dst + (off - lo), src.mem + off, len, cudaMemcpyHostToDevice, H.s_copy));
+		else {
+			CUDA_TRY(cudaEventSynchronize(H.ev[sb]));     /* that ring buffer has been consumed (by this call or an earlier one) */
+			if (!fill_slice(src, off, H.ring[sb], (size_t)len)) {
+				snprintf(g_err, sizeof g_err, "pread(2) failed or hit the end of the file in [%llu, %llu)", (unsigned long long)off, (unsigned long long)(off + len));
+				return AGB_ERR_ARG;
+			}
+			CUDA_TRY(cudaMemcpyAsync(dst + (off - lo), H.ring[sb], len, cudaMemcpyHostToDevice, H.s_copy));
+		}
+		CUDA_TRY(cudaEventRecord(H.ev[sb], H.s_copy));
+		if (after) { int rc = after(i, H.ev[sb]); if (rc) return rc; }
+	}
+	drain.on = false;
+	return AGB_OK;
 }
 
 /* AGB_MAX_TEXT_BYTES: the most bytes of text the library keeps on the device (0 or unset: no cap) */
@@ -687,81 +773,51 @@ static uint64_t max_text_bytes(void)
  * the caller scans it in windows instead */
 #define SCAN_NEEDS_WINDOWS 1
 
-static int scan_stream_impl(const agb_desc &d, const agb_regex *rx, uint64_t n, const SliceSource &src, int want,
+static int scan_stream_impl(const agb_desc &d, const agb_regex *rx, SliceSource &src, int want,
                             agb_record *records, uint64_t capacity, agb_result *res)
 {
 	memset(res, 0, sizeof *res);
 	int dev = 0; CUDA_TRY(cudaGetDevice(&dev));
 	if (dev < 0 || dev >= 64) return AGB_ERR_ARG;
+	std::lock_guard<std::mutex> hlk(g_host_mu[dev]);
 	std::lock_guard<std::mutex> lk(g_ws_mu[dev]);
+	HostPath &H = g_host[dev];
 	Workspace &W = g_ws[dev];
+	const uint64_t n = src.n;
 	const size_t need = (size_t)((n + 15) / 16 * 16 + 4096);
 	const uint64_t cap_bytes = max_text_bytes();
-	if (need > W.h2d_cap || (cap_bytes && need > cap_bytes)) {
-		if (W.h2d_text) cudaFree(W.h2d_text);
-		W.h2d_text = nullptr; W.h2d_cap = 0;
-		if (cap_bytes && need > cap_bytes) return SCAN_NEEDS_WINDOWS;
-		const cudaError_t e = cudaMalloc(&W.h2d_text, need);
-		if (e == cudaErrorMemoryAllocation) { cudaGetLastError(); W.h2d_text = nullptr; return SCAN_NEEDS_WINDOWS; }
-		CUDA_TRY(e); W.h2d_cap = need;
+	if (cap_bytes && need > cap_bytes) {
+		cudaFree(H.text); H.text = nullptr; H.text_cap = 0;       /* the cap holds between scans too */
+		return SCAN_NEEDS_WINDOWS;
 	}
+	const cudaError_t e = dev_reserve(&H.text, &H.text_cap, need);
+	if (e == cudaErrorMemoryAllocation) return SCAN_NEEDS_WINDOWS;
+	CUDA_TRY(e);
 	int rc = ws_prepare(W, n); if (rc) return rc;
-	if (!W.s_copy) {
-		CUDA_TRY(cudaStreamCreateWithFlags(&W.s_copy, cudaStreamNonBlocking));
-		CUDA_TRY(cudaStreamCreateWithFlags(&W.s_comp, cudaStreamNonBlocking));
-		for (int i = 0; i < STAGE_BUFS; i++) CUDA_TRY(cudaEventCreateWithFlags(&W.ev_copy[i], cudaEventDisableTiming));
-	}
-	if ((want & AGB_WANT_RECORDS) && capacity > W.h2d_rec_cap) {
-		if (W.h2d_rec) cudaFree(W.h2d_rec);
-		W.h2d_rec = nullptr; W.h2d_rec_cap = 0;
-		CUDA_TRY(cudaMalloc(&W.h2d_rec, capacity * sizeof(agb_record))); W.h2d_rec_cap = capacity;
-	}
-	rc = ws_upload_desc(W, d, W.s_comp); if (rc) return rc;
-	rc = regex_prepare(W, d, rx, W.s_comp); if (rc) return rc;
-	const bool direct = src.mem && src.pinned;
-	FdGuard dg; if (!src.mem && src.fd >= 0) dg.fd = open_direct(src.fd, src.fd_off);
-	int &dfd = dg.fd;
-	if (!direct && n && !W.stage[0]) for (int i = 0; i < STAGE_BUFS; i++) CUDA_TRY(cudaMallocHost(&W.stage[i], H2D_SLICE));
+	rc = host_ensure(H, src); if (rc) return rc;
+	CUDA_TRY(dev_reserve(&H.rec, &H.rec_cap, (want & AGB_WANT_RECORDS) ? capacity * sizeof(agb_record) : 0));
+	rc = ws_upload_desc(W, d, H.s_comp); if (rc) return rc;
+	rc = regex_prepare(W, d, rx, H.s_comp); if (rc) return rc;
 	const bool use_front = front_usable(d) && n > 0;
 	const bool count_in_front = use_front && (want & AGB_WANT_ORDINALS) && d.L == 1;
-	if (count_in_front) { rc = ordinals_prepare_blocks(d, W, n, W.s_comp); if (rc) return rc; }
+	if (count_in_front) { rc = ordinals_prepare_blocks(d, W, n, H.s_comp); if (rc) return rc; }
 	const uint64_t words_per_slice = H2D_SLICE / 512, n_slices = (n + H2D_SLICE - 1) / H2D_SLICE;
-	CUDA_TRY(cudaMemsetAsync(W.totals, 0, 16 * sizeof(unsigned long long), W.s_comp));
-	CUDA_TRY(cudaEventRecord(W.e0, W.s_comp));
-	/* zero the slack after the text once (stage 1 reads whole 16-byte chunks, stage 2 whole groups) */
-	CUDA_TRY(cudaMemsetAsync(W.h2d_text + (n & ~(uint64_t)15), 0, need - (n & ~(uint64_t)15), W.s_copy));
-	for (uint64_t i = 0; i < n_slices; i++) {
-		const uint64_t off = i * H2D_SLICE, len = std::min<uint64_t>(H2D_SLICE, n - off);
-		const int sb = (int)(i % STAGE_BUFS);
-		if (direct) {
-			CUDA_TRY(cudaMemcpyAsync(W.h2d_text + off, src.mem + off, len, cudaMemcpyHostToDevice, W.s_copy));
-		} else {
-			if (i >= STAGE_BUFS) CUDA_TRY(cudaEventSynchronize(W.ev_copy[sb]));     /* that staging buffer has been consumed */
-			if (src.mem) par_memcpy(W.stage[sb], src.mem + off, len);
-			else {
-				/* fill_buf(): the slice from the file */
-				if (!read_slice(src, &dfd, off, W.stage[sb], (size_t)len)) { snprintf(g_err, sizeof g_err, "pread(2) failed or hit the end of the file in [%llu, %llu) of %llu", (unsigned long long)off, (unsigned long long)(off + len), (unsigned long long)n); return AGB_ERR_ARG; }
-			}
-			CUDA_TRY(cudaMemcpyAsync(W.h2d_text + off, W.stage[sb], len, cudaMemcpyHostToDevice, W.s_copy));
-		}
-		CUDA_TRY(cudaEventRecord(W.ev_copy[sb], W.s_copy));
+	CUDA_TRY(cudaMemsetAsync(W.totals, 0, 16 * sizeof(unsigned long long), H.s_comp));
+	CUDA_TRY(cudaEventRecord(W.e0, H.s_comp));
+	rc = upload(H, src, 0, n, H.text, need - n, [&](uint64_t i, cudaEvent_t ev) -> int {
+		CUDA_TRY(cudaStreamWaitEvent(H.s_comp, ev, 0));
 		/* stage 1 on the previous slice: its last chunk looks 4 bytes into this one, which is now on its way */
-		if (use_front) {
-			CUDA_TRY(cudaStreamWaitEvent(W.s_comp, W.ev_copy[sb], 0));
-			if (i > 0) { rc = front_launch(d, W, W.h2d_text, n, (i - 1) * words_per_slice, i * words_per_slice, true, W.s_comp, count_in_front); if (rc) return rc; }
-		}
-	}
-	if (n_slices) {
-		CUDA_TRY(cudaStreamWaitEvent(W.s_comp, W.ev_copy[(n_slices - 1) % STAGE_BUFS], 0));
-		if (use_front) { rc = front_launch(d, W, W.h2d_text, n, (n_slices - 1) * words_per_slice, ~0ull, true, W.s_comp, count_in_front); if (rc) return rc; }
-	}
-	CUDA_TRY(cudaEventRecord(W.e1, W.s_comp));
-	rc = stages_after_front(d, W, W.h2d_text, n, use_front, count_in_front, want, -1, W.h2d_rec, capacity, W.s_comp, res); if (rc) return rc;
+		return use_front && i ? front_launch(d, W, H.text, n, (i - 1) * words_per_slice, i * words_per_slice, true, H.s_comp, count_in_front) : AGB_OK;
+	});
+	if (rc) return rc;
+	if (use_front) { rc = front_launch(d, W, H.text, n, (n_slices - 1) * words_per_slice, ~0ull, true, H.s_comp, count_in_front); if (rc) return rc; }
+	CUDA_TRY(cudaEventRecord(W.e1, H.s_comp));
+	rc = stages_after_front(d, W, H.text, n, use_front, count_in_front, want, -1, H.rec, capacity, H.s_comp, res); if (rc) return rc;
 	if (res->n_records) {
-		CUDA_TRY(cudaMemcpyAsync(records, W.h2d_rec, res->n_records * sizeof(agb_record), cudaMemcpyDeviceToHost, W.s_comp));
-		CUDA_TRY(cudaStreamSynchronize(W.s_comp));
+		CUDA_TRY(cudaMemcpyAsync(records, H.rec, res->n_records * sizeof(agb_record), cudaMemcpyDeviceToHost, H.s_comp));
+		CUDA_TRY(cudaStreamSynchronize(H.s_comp));
 	}
-	CUDA_TRY(cudaStreamSynchronize(W.s_copy));
+	CUDA_TRY(cudaStreamSynchronize(H.s_copy));
 	CUDA_TRY(cudaEventElapsedTime(&res->ms_front, W.e0, W.e1));
 	CUDA_TRY(cudaEventElapsedTime(&res->ms_records, W.e1, W.e2));
 	return AGB_OK;
@@ -777,60 +833,14 @@ static int scan_stream_impl(const agb_desc &d, const agb_regex *rx, uint64_t n, 
  * Counts and histograms are summed; each window's records are made global on the device and appended to the caller's
  * list until it is full; the ordinals follow the gather's arithmetic (agb_shard_part).
  * ---------------------------------------------------------------------------------------------- */
-struct WinState {                 /* per device, kept across calls: streams and the pinned ring (device buffers live for one call) */
-	cudaStream_t s_copy = nullptr, s_comp = nullptr;
-	cudaEvent_t ev[STAGE_BUFS] = {nullptr, nullptr, nullptr};
-	uint8_t *stage[STAGE_BUFS] = {nullptr, nullptr, nullptr};
-};
-static WinState g_win[64];
-static std::mutex g_win_mu[64];   /* one windowed scan at a time per device; taken before (never inside) g_ws_mu */
-
-static void win_release(int dev)
-{
-	std::lock_guard<std::mutex> lk(g_win_mu[dev]);
-	WinState &S = g_win[dev];
-	if (!S.s_copy) return;
-	if (cudaSetDevice(dev) != cudaSuccess) { cudaGetLastError(); return; }
-	cudaStreamSynchronize(S.s_copy); cudaStreamSynchronize(S.s_comp);
-	for (int i = 0; i < STAGE_BUFS; i++) { if (S.ev[i]) cudaEventDestroy(S.ev[i]); if (S.stage[i]) cudaFreeHost(S.stage[i]); }
-	cudaStreamDestroy(S.s_copy); cudaStreamDestroy(S.s_comp);
-	S = WinState();
-}
-
 /* device memory of one windowed scan */
 struct WinBuffers {
 	uint8_t *buf[2] = {nullptr, nullptr}, *big = nullptr; size_t big_cap = 0;
-	agb_record *rec = nullptr; uint64_t rec_cap = 0;
+	agb_record *rec = nullptr; size_t rec_cap = 0;          /* (capacities in bytes) */
 	~WinBuffers() { cudaFree(buf[0]); cudaFree(buf[1]); cudaFree(big); cudaFree(rec); }
 };
 
 #define WIN_SLACK 4096            /* zeroed bytes behind a window's scanned range, as behind a whole text */
-
-/* bytes [lo, hi) of the source to dst on the device, then WIN_SLACK zero bytes; returns once they are there */
-static int upload_range(const SliceSource &src, int *dfd, WinState &S, uint64_t lo, uint64_t hi, uint8_t *dst)
-{
-	const bool direct = src.mem && src.pinned;
-	uint64_t i = 0;
-	for (uint64_t off = lo; off < hi; off += H2D_SLICE, i++) {
-		const uint64_t len = std::min<uint64_t>(H2D_SLICE, hi - off);
-		const int sb = (int)(i % STAGE_BUFS);
-		if (direct) { CUDA_TRY(cudaMemcpyAsync(dst + (off - lo), src.mem + off, len, cudaMemcpyHostToDevice, S.s_copy)); continue; }
-		if (i >= STAGE_BUFS) CUDA_TRY(cudaEventSynchronize(S.ev[sb]));          /* that staging buffer has been consumed */
-		if (src.mem) {
-			if (len < (1u << 20)) memcpy(S.stage[sb], src.mem + off, len);     /* (small windows: four threads cost more than they save) */
-			else par_memcpy(S.stage[sb], src.mem + off, len);
-		} else if (!read_slice(src, dfd, off, S.stage[sb], (size_t)len)) {
-			cudaStreamSynchronize(S.s_copy);
-			snprintf(g_err, sizeof g_err, "pread(2) failed or hit the end of the file in [%llu, %llu)", (unsigned long long)off, (unsigned long long)(off + len));
-			return AGB_ERR_ARG;
-		}
-		CUDA_TRY(cudaMemcpyAsync(dst + (off - lo), S.stage[sb], len, cudaMemcpyHostToDevice, S.s_copy));
-		CUDA_TRY(cudaEventRecord(S.ev[sb], S.s_copy));
-	}
-	CUDA_TRY(cudaMemsetAsync(dst + (hi - lo), 0, WIN_SLACK, S.s_copy));
-	CUDA_TRY(cudaStreamSynchronize(S.s_copy));
-	return AGB_OK;
-}
 
 /* window i with halos of (at most) hl and hr bytes */
 struct WinGeom { uint64_t a, n_local, hl, hr, lo, hi; bool first, open_end, reaches_end; };
@@ -846,36 +856,28 @@ static WinGeom win_geom(uint64_t n, uint64_t w, uint64_t i, uint64_t hl, uint64_
 	return g;
 }
 
-static int scan_windowed(const agb_desc &d, const agb_regex *rx, uint64_t n, const SliceSource &src, uint64_t w, int want,
+static int scan_windowed(const agb_desc &d, const agb_regex *rx, SliceSource &src, uint64_t w, int want,
                          agb_record *records, uint64_t capacity, agb_result *res)
 {
 	memset(res, 0, sizeof *res);
 	int dev = 0; CUDA_TRY(cudaGetDevice(&dev));
 	if (dev < 0 || dev >= 64) return AGB_ERR_ARG;
-	std::lock_guard<std::mutex> lk(g_win_mu[dev]);
-	WinState &S = g_win[dev];
-	if (!S.s_copy) {
-		CUDA_TRY(cudaStreamCreateWithFlags(&S.s_copy, cudaStreamNonBlocking));
-		CUDA_TRY(cudaStreamCreateWithFlags(&S.s_comp, cudaStreamNonBlocking));
-		for (int i = 0; i < STAGE_BUFS; i++) CUDA_TRY(cudaEventCreateWithFlags(&S.ev[i], cudaEventDisableTiming));
-	}
-	if (!(src.mem && src.pinned) && n && !S.stage[0]) for (int i = 0; i < STAGE_BUFS; i++) CUDA_TRY(cudaMallocHost(&S.stage[i], H2D_SLICE));
+	std::lock_guard<std::mutex> lk(g_host_mu[dev]);
+	HostPath &H = g_host[dev];
+	int rc = host_ensure(H, src); if (rc) return rc;
+	const uint64_t n = src.n;
 	const bool want_list = (want & AGB_WANT_RECORDS) && capacity, ord = (want & AGB_WANT_ORDINALS) != 0;
 	WinBuffers B;
 	const size_t buf_bytes = std::min<uint64_t>(n, w + AGB_HALO_LEFT + AGB_HALO_RIGHT) + WIN_SLACK;
 	for (int b = 0; b < 2; b++) CUDA_TRY(cudaMalloc(&B.buf[b], buf_bytes));
-	if (want_list) {
-		/* most windows own far fewer records than bytes; one that owns more is scanned again with a longer list */
-		B.rec_cap = std::min<uint64_t>(capacity, w / 256 + 4096);
-		CUDA_TRY(cudaMalloc(&B.rec, B.rec_cap * sizeof(agb_record)));
-	}
-	FdGuard dg; if (!src.mem && src.fd >= 0) dg.fd = open_direct(src.fd, src.fd_off);
-	int &dfd = dg.fd;
+	/* most windows own far fewer records than bytes; one that owns more is scanned again with a longer list */
+	if (want_list) CUDA_TRY(dev_reserve(&B.rec, &B.rec_cap, std::min<uint64_t>(capacity, w / 256 + 4096) * sizeof(agb_record)));
 	const uint64_t m = n ? (n + w - 1) / w : 1;
-	int rc = upload_range(src, &dfd, S, 0, win_geom(n, w, 0, AGB_HALO_LEFT, AGB_HALO_RIGHT).hi, B.buf[0]); if (rc) return rc;
+	rc = upload(H, src, 0, win_geom(n, w, 0, AGB_HALO_LEFT, AGB_HALO_RIGHT).hi, B.buf[0], WIN_SLACK); if (rc) return rc;
+	CUDA_TRY(cudaStreamSynchronize(H.s_copy));
 	uint64_t copied = 0; long long origin = 0, closes_before = 0;
 	for (uint64_t i = 0; i < m; i++) {
-		/* the next window on its way while this one is scanned (the thread has the pinned ring and dfd to itself until joined) */
+		/* the next window on its way while this one is scanned (the thread has the pinned ring and src.dfd to itself until joined) */
 		int up_rc = AGB_OK; char up_err[sizeof g_err] = "";
 		std::thread up;
 		struct Joiner { std::thread &t; ~Joiner() { if (t.joinable()) t.join(); } } joiner{up};   /* every way out of this iteration */
@@ -883,13 +885,14 @@ static int scan_windowed(const agb_desc &d, const agb_regex *rx, uint64_t n, con
 			const WinGeom gn = win_geom(n, w, i + 1, AGB_HALO_LEFT, AGB_HALO_RIGHT);
 			uint8_t *dst = B.buf[(i + 1) & 1];
 			up = std::thread([&, gn, dst] {
-				up_rc = cudaSetDevice(dev) == cudaSuccess ? upload_range(src, &dfd, S, gn.lo, gn.hi, dst) : AGB_ERR_CUDA;
+				up_rc = cudaSetDevice(dev) == cudaSuccess ? upload(H, src, gn.lo, gn.hi, dst, WIN_SLACK) : AGB_ERR_CUDA;
 				if (up_rc) memcpy(up_err, g_err, sizeof up_err);     /* (g_err is per thread) */
 			});
 		}
-		auto join_up = [&]() -> int {
+		auto join_up = [&]() -> int {           /* the next window's bytes on the device, the ring free */
 			if (up.joinable()) up.join();
 			if (up_rc) { memcpy(g_err, up_err, sizeof up_err); return up_rc; }
+			CUDA_TRY(cudaStreamSynchronize(H.s_copy));
 			return AGB_OK;
 		};
 		uint64_t hl = AGB_HALO_LEFT, hr = AGB_HALO_RIGHT;
@@ -897,18 +900,16 @@ static int scan_windowed(const agb_desc &d, const agb_regex *rx, uint64_t n, con
 		WinGeom g; agb_result lres; agb_shard_part part;
 		for (;;) {
 			g = win_geom(n, w, i, hl, hr);
-			const uint64_t room = want_list ? std::min<uint64_t>(capacity - copied, B.rec_cap) : 0;
+			const uint64_t room = want_list ? std::min<uint64_t>(capacity - copied, B.rec_cap / sizeof(agb_record)) : 0;
 			rc = shard_window_scan(d, rx, base + g.hl, g.n_local, g.hl, g.hr, g.first, g.open_end, g.reaches_end, want,
-			                       B.rec, room, S.s_comp, &lres, &part);
+			                       B.rec, room, H.s_comp, &lres, &part);
 			if (rc < 0) return rc;
 			int short_halos = rc;
 			if (g.lo == 0) short_halos &= ~HALO_SHORT_LEFT;      /* the scan starts where the text does: a run there really begins there */
 			if (!short_halos) {
 				if (!(want_list && lres.n_matched > room && room < capacity - copied)) break;
 				/* more records than the list had room for, and the caller's list has more: again with room for all of them */
-				cudaFree(B.rec); B.rec = nullptr;
-				B.rec_cap = std::min<uint64_t>(capacity - copied, lres.n_matched);
-				CUDA_TRY(cudaMalloc(&B.rec, B.rec_cap * sizeof(agb_record)));
+				CUDA_TRY(dev_reserve(&B.rec, &B.rec_cap, std::min<uint64_t>(capacity - copied, lres.n_matched) * sizeof(agb_record)));
 				continue;
 			}
 			if (short_halos & HALO_SHORT_LEFT) hl *= 2;
@@ -916,18 +917,14 @@ static int scan_windowed(const agb_desc &d, const agb_regex *rx, uint64_t n, con
 			g = win_geom(n, w, i, hl, hr);
 			rc = join_up(); if (rc) return rc;                      /* the ring is needed here */
 			const size_t need = g.hi - g.lo + WIN_SLACK;
-			if (need > B.big_cap) {
-				cudaFree(B.big); B.big = nullptr; B.big_cap = 0;
-				const cudaError_t e = cudaMalloc(&B.big, need);
-				if (e != cudaSuccess) {
-					cudaGetLastError();
-					snprintf(g_err, sizeof g_err, "a record that begins in bytes [%llu, %llu) of the text does not fit in device memory with its halos (%llu bytes: %s)",
-					         (unsigned long long)g.a, (unsigned long long)(g.a + g.n_local), (unsigned long long)need, cudaGetErrorString(e));
-					return e == cudaErrorMemoryAllocation ? AGB_ERR_NOMEM : AGB_ERR_CUDA;
-				}
-				B.big_cap = need;
+			const cudaError_t e = dev_reserve(&B.big, &B.big_cap, need);
+			if (e != cudaSuccess) {
+				snprintf(g_err, sizeof g_err, "a record that begins in bytes [%llu, %llu) of the text does not fit in device memory with its halos (%llu bytes: %s)",
+				         (unsigned long long)g.a, (unsigned long long)(g.a + g.n_local), (unsigned long long)need, cudaGetErrorString(e));
+				return e == cudaErrorMemoryAllocation ? AGB_ERR_NOMEM : AGB_ERR_CUDA;
 			}
-			rc = upload_range(src, &dfd, S, g.lo, g.hi, B.big); if (rc) return rc;
+			rc = upload(H, src, g.lo, g.hi, B.big, WIN_SLACK); if (rc) return rc;
+			CUDA_TRY(cudaStreamSynchronize(H.s_copy));
 			base = B.big;
 		}
 		res->n_matched += lres.n_matched; res->n_flagged += lres.n_flagged;
@@ -936,10 +933,10 @@ static int scan_windowed(const agb_desc &d, const agb_regex *rx, uint64_t n, con
 		if (ord && i == 0) { origin = part.ord_origin; res->n_closes += (uint64_t)part.virt; }
 		if (lres.n_records) {
 			/* offsets: local to the scanned range, which starts at g.lo = g.a + part.byte_base; ordinals as the gather makes them */
-			rc = shard_window_rebase(B.rec, lres.n_records, (long long)g.a + part.byte_base, origin + closes_before - part.ord_fix, ord, S.s_comp);
+			rc = shard_window_rebase(B.rec, lres.n_records, (long long)g.a + part.byte_base, origin + closes_before - part.ord_fix, ord, H.s_comp);
 			if (rc) return rc;
-			CUDA_TRY(cudaMemcpyAsync(records + copied, B.rec, lres.n_records * sizeof(agb_record), cudaMemcpyDeviceToHost, S.s_comp));
-			CUDA_TRY(cudaStreamSynchronize(S.s_comp));
+			CUDA_TRY(cudaMemcpyAsync(records + copied, B.rec, lres.n_records * sizeof(agb_record), cudaMemcpyDeviceToHost, H.s_comp));
+			CUDA_TRY(cudaStreamSynchronize(H.s_comp));
 			copied += lres.n_records;
 		}
 		if (ord) { closes_before += (long long)part.closes; res->n_closes += part.closes; }
@@ -965,25 +962,16 @@ static uint64_t fallback_window(void)
 	return budget / 2 >= per + 4096 ? (budget / 2 - per) & ~(uint64_t)511 : 4096;
 }
 
-static bool host_pinned(const void *h_text, uint64_t n)
-{
-	if (!n) return false;
-	cudaPointerAttributes attr; memset(&attr, 0, sizeof attr);
-	const bool pinned = cudaPointerGetAttributes(&attr, h_text) == cudaSuccess && attr.type == cudaMemoryTypeHost;
-	cudaGetLastError();
-	return pinned;
-}
-
 /* window_bytes == 0: the whole text on the device when it fits, windows when it does not */
 static int scan_host_any(const agb_pattern *p, const void *h_text, uint64_t n, uint64_t window_bytes, int want,
                          agb_record *records, uint64_t capacity, agb_result *res)
 {
 	if (!p || !res || (!h_text && n)) return AGB_ERR_ARG;
 	if ((want & AGB_WANT_RECORDS) && capacity && !records) return AGB_ERR_ARG;
-	SliceSource src; src.mem = (const uint8_t *)h_text; src.fd = -1; src.pinned = host_pinned(h_text, n);
-	if (window_bytes) return scan_windowed(p->d, agb_pattern_regex(p), n, src, window_bytes, want, records, capacity, res);
-	int rc = scan_stream_impl(p->d, agb_pattern_regex(p), n, src, want, records, capacity, res);
-	if (rc == SCAN_NEEDS_WINDOWS) rc = scan_windowed(p->d, agb_pattern_regex(p), n, src, fallback_window(), want, records, capacity, res);
+	SliceSource src(h_text, n);
+	if (window_bytes) return scan_windowed(p->d, agb_pattern_regex(p), src, window_bytes, want, records, capacity, res);
+	int rc = scan_stream_impl(p->d, agb_pattern_regex(p), src, want, records, capacity, res);
+	if (rc == SCAN_NEEDS_WINDOWS) rc = scan_windowed(p->d, agb_pattern_regex(p), src, fallback_window(), want, records, capacity, res);
 	return rc;
 }
 
@@ -991,16 +979,13 @@ static int scan_fd_any(const agb_pattern *p, int fd, uint64_t window_bytes, int 
 {
 	if (!p || !res) return AGB_ERR_ARG;
 	if ((want & AGB_WANT_RECORDS) && capacity && !records) return AGB_ERR_ARG;
-	struct stat sb;
-	if (fstat(fd, &sb) == 0 && S_ISREG(sb.st_mode)) {
+	SliceSource src;
+	if (fd_source(fd, src)) {
 		/* regular file: the size is known, read(2) goes straight into the pinned ring, slice by slice */
-		off_t cur = lseek(fd, 0, SEEK_CUR);
-		uint64_t n = (cur >= 0 && sb.st_size > cur) ? (uint64_t)(sb.st_size - cur) : 0;
-		SliceSource src; src.mem = nullptr; src.pinned = false; src.fd = fd; src.fd_off = cur >= 0 ? cur : 0;
-		int rc = window_bytes ? scan_windowed(p->d, agb_pattern_regex(p), n, src, window_bytes, want, records, capacity, res)
-		                      : scan_stream_impl(p->d, agb_pattern_regex(p), n, src, want, records, capacity, res);
-		if (rc == SCAN_NEEDS_WINDOWS) rc = scan_windowed(p->d, agb_pattern_regex(p), n, src, fallback_window(), want, records, capacity, res);
-		if (cur >= 0) lseek(fd, cur + (off_t)n, SEEK_SET);            /* as read(2) would have left it */
+		int rc = window_bytes ? scan_windowed(p->d, agb_pattern_regex(p), src, window_bytes, want, records, capacity, res)
+		                      : scan_stream_impl(p->d, agb_pattern_regex(p), src, want, records, capacity, res);
+		if (rc == SCAN_NEEDS_WINDOWS) rc = scan_windowed(p->d, agb_pattern_regex(p), src, fallback_window(), want, records, capacity, res);
+		if (src.fd_off >= 0) lseek(fd, src.fd_off + (off_t)src.n, SEEK_SET);        /* as read(2) would have left it */
 		return rc;
 	}
 	/* pipes, ttys: fill_buf() semantics -- read until EOF into a growing buffer, then as host memory */
@@ -1054,10 +1039,11 @@ extern "C" int agb_scan_fd_windowed(const agb_pattern *p, int fd, uint64_t windo
  * agrep.c:3582-3728: one upload instead of K + 2) ---- */
 struct agb_text { uint8_t *d; uint64_t n; int dev; };
 
-static int text_upload(const SliceSource &src, uint64_t n, agb_text **out)
+static int text_upload(SliceSource &src, agb_text **out)
 {
 	int dev = 0; CUDA_TRY(cudaGetDevice(&dev));
 	if (dev < 0 || dev >= 64) return AGB_ERR_ARG;
+	const uint64_t n = src.n;
 	const size_t need = (size_t)((n + 15) / 16 * 16 + 4096);
 	const uint64_t cap_bytes = max_text_bytes();
 	if (cap_bytes && need > cap_bytes) {
@@ -1065,64 +1051,32 @@ static int text_upload(const SliceSource &src, uint64_t n, agb_text **out)
 		         (unsigned long long)n, (unsigned long long)cap_bytes);
 		return AGB_ERR_NOMEM;
 	}
-	agb_text *t = new agb_text; t->d = nullptr; t->n = n; t->dev = dev;
-	if (cudaMalloc(&t->d, need) != cudaSuccess) { delete t; snprintf(g_err, sizeof g_err, "cudaMalloc of %zu bytes for the text failed", need); cudaGetLastError(); return AGB_ERR_NOMEM; }
-	std::lock_guard<std::mutex> lk(g_ws_mu[dev]);
-	Workspace &W = g_ws[dev];
-	int rc = ws_prepare(W, 0); if (rc) { cudaFree(t->d); delete t; return rc; }
-	if (!W.s_copy) {
-		CUDA_TRY(cudaStreamCreateWithFlags(&W.s_copy, cudaStreamNonBlocking));
-		CUDA_TRY(cudaStreamCreateWithFlags(&W.s_comp, cudaStreamNonBlocking));
-		for (int i = 0; i < STAGE_BUFS; i++) CUDA_TRY(cudaEventCreateWithFlags(&W.ev_copy[i], cudaEventDisableTiming));
-	}
-	const bool direct = src.mem && src.pinned;
-	FdGuard dg; if (!src.mem && src.fd >= 0) dg.fd = open_direct(src.fd, src.fd_off);
-	int &dfd = dg.fd;
-	if (!direct && n && !W.stage[0]) for (int i = 0; i < STAGE_BUFS; i++) CUDA_TRY(cudaMallocHost(&W.stage[i], H2D_SLICE));
-	CUDA_TRY(cudaMemsetAsync(t->d + (n & ~(uint64_t)15), 0, need - (n & ~(uint64_t)15), W.s_copy));
-	const uint64_t n_slices = (n + H2D_SLICE - 1) / H2D_SLICE;
-	for (uint64_t i = 0; i < n_slices; i++) {
-		const uint64_t off = i * H2D_SLICE, len = std::min<uint64_t>(H2D_SLICE, n - off);
-		const int sb = (int)(i % STAGE_BUFS);
-		if (direct) CUDA_TRY(cudaMemcpyAsync(t->d + off, src.mem + off, len, cudaMemcpyHostToDevice, W.s_copy));
-		else {
-			if (i >= STAGE_BUFS) CUDA_TRY(cudaEventSynchronize(W.ev_copy[sb]));
-			if (src.mem) par_memcpy(W.stage[sb], src.mem + off, len);
-			else {
-				if (!read_slice(src, &dfd, off, W.stage[sb], (size_t)len)) { snprintf(g_err, sizeof g_err, "pread(2) failed or hit the end of the file in [%llu, %llu) of %llu", (unsigned long long)off, (unsigned long long)(off + len), (unsigned long long)n); cudaStreamSynchronize(W.s_copy); cudaFree(t->d); delete t; return AGB_ERR_ARG; }
-			}
-			CUDA_TRY(cudaMemcpyAsync(t->d + off, W.stage[sb], len, cudaMemcpyHostToDevice, W.s_copy));
-		}
-		CUDA_TRY(cudaEventRecord(W.ev_copy[sb], W.s_copy));
-	}
-	CUDA_TRY(cudaStreamSynchronize(W.s_copy));
-	*out = t;
+	std::unique_ptr<agb_text, decltype(&agb_text_free)> t(new agb_text{nullptr, n, dev}, agb_text_free);   /* freed on every error exit */
+	if (cudaMalloc(&t->d, need) != cudaSuccess) { t->d = nullptr; snprintf(g_err, sizeof g_err, "cudaMalloc of %zu bytes for the text failed", need); cudaGetLastError(); return AGB_ERR_NOMEM; }
+	std::lock_guard<std::mutex> lk(g_host_mu[dev]);
+	HostPath &H = g_host[dev];
+	int rc = host_ensure(H, src); if (rc) return rc;
+	rc = upload(H, src, 0, n, t->d, need - n); if (rc) return rc;
+	CUDA_TRY(cudaStreamSynchronize(H.s_copy));
+	*out = t.release();
 	return AGB_OK;
 }
 
 extern "C" int agb_text_from_host(const void *h_text, uint64_t n, agb_text **out)
 {
 	if (!out || (!h_text && n)) return AGB_ERR_ARG;
-	SliceSource src; src.mem = (const uint8_t *)h_text; src.fd = -1; src.pinned = false;
-	if (n) {
-		cudaPointerAttributes attr; memset(&attr, 0, sizeof attr);
-		src.pinned = cudaPointerGetAttributes(&attr, h_text) == cudaSuccess && attr.type == cudaMemoryTypeHost;
-		cudaGetLastError();
-	}
-	return text_upload(src, n, out);
+	SliceSource src(h_text, n);
+	return text_upload(src, out);
 }
 
 extern "C" int agb_text_from_fd(int fd, agb_text **out)
 {
 	if (!out) return AGB_ERR_ARG;
-	struct stat sb;
-	if (fstat(fd, &sb) != 0 || !S_ISREG(sb.st_mode)) { snprintf(g_err, sizeof g_err, "agb_text_from_fd needs a regular file"); return AGB_ERR_ARG; }
-	off_t cur = lseek(fd, 0, SEEK_CUR);
-	const uint64_t n = (cur >= 0 && sb.st_size > cur) ? (uint64_t)(sb.st_size - cur) : 0;
-	SliceSource src; src.mem = nullptr; src.pinned = false; src.fd = fd; src.fd_off = cur >= 0 ? cur : 0;
-	int rc = text_upload(src, n, out);
+	SliceSource src;
+	if (!fd_source(fd, src)) { snprintf(g_err, sizeof g_err, "agb_text_from_fd needs a regular file"); return AGB_ERR_ARG; }
+	int rc = text_upload(src, out);
 	/* as read(2) would have left it; untouched when the text was not taken, so that the caller can read it another way */
-	if (cur >= 0) lseek(fd, rc == AGB_OK ? cur + (off_t)n : cur, SEEK_SET);
+	if (src.fd_off >= 0) lseek(fd, src.fd_off + (rc == AGB_OK ? (off_t)src.n : 0), SEEK_SET);
 	return rc;
 }
 
@@ -1131,31 +1085,17 @@ extern "C" uint64_t agb_text_size(const agb_text *t) { return t ? t->n : 0; }
 extern "C" const void *agb_text_device(const agb_text *t) { return t ? t->d : nullptr; }
 
 /* device scan of a resident text with the record list delivered to host memory */
-static int scan_text_impl(const agb_desc &d, const agb_regex *rx, const agb_text *t, int want, int want_level, agb_record *records, uint64_t capacity, agb_result *res)
-{
-	if (!t || !res) return AGB_ERR_ARG;
-	if ((want & AGB_WANT_RECORDS) && capacity && !records) return AGB_ERR_ARG;
-	CUDA_TRY(cudaSetDevice(t->dev));
-	agb_record *d_rec = nullptr;
-	{
-		std::lock_guard<std::mutex> lk(g_ws_mu[t->dev]);
-		Workspace &W = g_ws[t->dev];
-		if ((want & AGB_WANT_RECORDS) && capacity > W.h2d_rec_cap) {
-			if (W.h2d_rec) cudaFree(W.h2d_rec);
-			W.h2d_rec = nullptr; W.h2d_rec_cap = 0;
-			CUDA_TRY(cudaMalloc(&W.h2d_rec, capacity * sizeof(agb_record))); W.h2d_rec_cap = capacity;
-		}
-		d_rec = W.h2d_rec;
-	}
-	int rc = scan_device_impl(d, t->d, t->n, want, want_level, d_rec, capacity, nullptr, res, nullptr, rx); if (rc) return rc;
-	if (res->n_records) CUDA_TRY(cudaMemcpy(records, d_rec, res->n_records * sizeof(agb_record), cudaMemcpyDeviceToHost));
-	return AGB_OK;
-}
-
 extern "C" int agb_scan_text(const agb_pattern *p, const agb_text *t, int want, agb_record *records, uint64_t capacity, agb_result *res)
 {
-	if (!p) return AGB_ERR_ARG;
-	return scan_text_impl(p->d, agb_pattern_regex(p), t, want, -1, records, capacity, res);
+	if (!p || !t || !res) return AGB_ERR_ARG;
+	if ((want & AGB_WANT_RECORDS) && capacity && !records) return AGB_ERR_ARG;
+	CUDA_TRY(cudaSetDevice(t->dev));
+	std::lock_guard<std::mutex> lk(g_host_mu[t->dev]);
+	HostPath &H = g_host[t->dev];
+	CUDA_TRY(dev_reserve(&H.rec, &H.rec_cap, (want & AGB_WANT_RECORDS) ? capacity * sizeof(agb_record) : 0));
+	int rc = scan_device_impl(p->d, t->d, t->n, want, -1, H.rec, capacity, nullptr, res, nullptr, agb_pattern_regex(p)); if (rc) return rc;
+	if (res->n_records) CUDA_TRY(cudaMemcpy(records, H.rec, res->n_records * sizeof(agb_record), cudaMemcpyDeviceToHost));
+	return AGB_OK;
 }
 
 /* keep the records of one level (stable, in place: the output index never overtakes the input index) */

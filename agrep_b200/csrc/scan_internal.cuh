@@ -168,12 +168,6 @@ struct Workspace {               /* grow-only device scratch, one per device */
 	agb_desc *d_desc = nullptr; agb_desc h_desc_copy; bool desc_valid = false;
 	cudaEvent_t e0 = nullptr, e1 = nullptr, e2 = nullptr;
 	int sm_count = 0;
-	/* agb_scan_host: device copy of the text, record buffer, copy stream, pinned staging for pageable sources */
-	uint8_t *h2d_text = nullptr; size_t h2d_cap = 0;
-	agb_record *h2d_rec = nullptr; size_t h2d_rec_cap = 0;
-	cudaStream_t s_copy = nullptr, s_comp = nullptr;
-	cudaEvent_t ev_copy[STAGE_BUFS] = {nullptr, nullptr, nullptr};
-	uint8_t *stage[STAGE_BUFS] = {nullptr, nullptr, nullptr};
 	/* the Next tables of the last regular expression scanned (regex.cu), and their host copy */
 	uint64_t *d_regex = nullptr; uint64_t h_regex[8 * 256]; size_t regex_bytes = 0; int regex_tail = 0;
 };
