@@ -61,7 +61,7 @@ class CorpusSpec(C.Structure):
 
 EXPORTS = ["agb_fill_ordinals", "agb_compile", "agb_pattern_free", "agb_pattern_desc", "agb_pattern_from_desc", "agb_scan_device",
            "agb_pattern_regex", "agb_pattern_from_regex",
-           "agb_scan_host", "agb_scan_fd", "agb_scan_host_windowed", "agb_scan_fd_windowed", "agb_bestmatch_device", "agb_corpus_fill_device", "agb_corpus_fill_host",
+           "agb_scan_host", "agb_scan_fd", "agb_scan_host_windowed", "agb_scan_fd_windowed", "agb_scan_set", "agb_bestmatch_device", "agb_corpus_fill_device", "agb_corpus_fill_host",
            "agb_last_error", "agb_device_count", "agb_set_device", "agb_version", "agb_kernel_launches", "agb_shutdown",
            "agb_text_from_host", "agb_text_from_fd", "agb_text_free", "agb_text_size", "agb_text_device", "agb_scan_text",
            "agb_comm_unique_id", "agb_comm_init", "agb_comm_free", "agb_comm_world", "agb_comm_rank", "agb_shard_halo",
@@ -101,6 +101,8 @@ def lib():
     L.agb_scan_fd.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint64, C.POINTER(Result)]
     L.agb_scan_host_windowed.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int, C.c_void_p, C.c_uint64, C.POINTER(Result)]
     L.agb_scan_fd_windowed.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_int, C.c_void_p, C.c_uint64, C.POINTER(Result)]
+    L.agb_scan_set.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.c_uint32, C.c_int, C.c_void_p, C.c_uint64,
+                               C.POINTER(Result), C.POINTER(Result)]
     L.agb_bestmatch_device.argtypes = [C.c_char_p, C.POINTER(Options), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64,
                                        C.POINTER(C.c_int), C.POINTER(Result), C.c_char_p, C.c_size_t]
     L.agb_corpus_fill_device.argtypes = [C.POINTER(CorpusSpec), C.c_void_p, C.c_void_p]

@@ -115,6 +115,27 @@ class Pattern:
             os.lseek(fd, start, os.SEEK_SET)
             cap = res.n_matched
 
+    def scan_set(self, texts, want_records=True, capacity=None, levels=False, ordinals=False):
+        """texts: a list of bytes-like host texts, scanned in one device pass (agb_scan_set), each as if alone.
+        Returns (total Result, [Result per text], records) -- records as scan_host's tuples with the text's index last,
+        file 0's first; offsets and ordinals relative to the record's own text.  capacity: as in scan_host, over the set."""
+        nf = len(texts)
+        want = (WANT_RECORDS if want_records else WANT_COUNT) | (WANT_LEVELS if levels else 0) | (WANT_ORDINALS if ordinals else 0)
+        bufs = [(C.c_char * len(t)).from_buffer_copy(t) if len(t) else None for t in texts]
+        ptrs = (C.c_void_p * nf)(*[C.cast(b, C.c_void_p) if b is not None else None for b in bufs]) if nf else None
+        sizes = (C.c_uint64 * nf)(*[len(t) for t in texts]) if nf else None
+        cap = (capacity if capacity is not None else sum(len(t) for t in texts) // 64 + 4096) if want_records else 0
+        while True:
+            recs = (Record * cap)() if cap else None
+            total, per = Result(), ((Result * nf)() if nf else None)
+            rc = _lib.lib().agb_scan_set(self._h, ptrs, sizes, nf, want, recs, cap, per, C.byref(total))
+            if rc != 0:
+                raise AgrepError("agb_scan_set rc=%d: %s" % (rc, _lib.lib().agb_last_error().decode()))
+            if not total.truncated or capacity is not None:
+                out = [(recs[i].begin, recs[i].end, recs[i].ordinal, recs[i].level, recs[i].pad) for i in range(total.n_records)]
+                return total, (list(per) if nf else []), out
+            cap = total.n_matched
+
     def scan_device(self, dev_ptr, n, stream=0, d_records=0, capacity=0, levels=False, ordinals=False):
         """dev_ptr: device address of n bytes (16-byte aligned, e.g. torch tensor .data_ptr())."""
         want = (WANT_RECORDS if capacity else WANT_COUNT) | (WANT_LEVELS if levels else 0) | (WANT_ORDINALS if ordinals else 0)

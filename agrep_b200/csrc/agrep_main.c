@@ -36,10 +36,18 @@ static int is_regex(const char *s)
 	return 0;
 }
 
-static unsigned char *slurp(const char *path, size_t *n, int L, const unsigned char *dpat)
+static void cannot_open(const char *path)
+{
+	if (!QUIET_OPEN) fprintf(stderr, "%s: can't open file for reading: %s\n", prog, path);
+}
+
+/* the file with the virtual newline in front and the delimiter behind; NULL with *unopened set when it cannot be opened
+ * (the caller says so once the output of the files before it is out) */
+static unsigned char *slurp(const char *path, size_t *n, int L, const unsigned char *dpat, int *unopened)
 {
 	int fd = path ? open(path, O_RDONLY) : 0; struct stat sb; size_t cap, len = 0; unsigned char *b;
-	if (fd < 0) { if (!QUIET_OPEN) fprintf(stderr, "%s: can't open file for reading: %s\n", prog, path); return NULL; }
+	*unopened = fd < 0;
+	if (fd < 0) return NULL;
 	cap = (fstat(fd, &sb) == 0 && S_ISREG(sb.st_mode)) ? (size_t)sb.st_size + 1 : (1u << 20);
 	b = (unsigned char *)malloc(cap + 64);
 	if (!b) { if (path) close(fd); return NULL; }
@@ -84,40 +92,102 @@ static void print_record(const unsigned char *hb, const agb_desc *d, const agb_r
 	if (i1 <= i2) fwrite(hb + i1, 1, (size_t)(i2 - i1 + 1), stdout);
 }
 
+/* what exec() does with one file's scan result (agrep.c:3411-3576): the histogram of a levels pass, the count, the records,
+ * the -c / -l lines */
+static void finish_file(const agb_desc *d, const char *fname, const unsigned char *hb, const agb_result *res, const agb_record *recs,
+                        int counting, unsigned long long *hist)
+{
+	const int before = num_of_matched, count_only = counting || COUNT || SILENT || FILENAMEONLY;
+	size_t i;
+	if (hist) { for (i = 0; i <= AGB_MAXERR; i++) hist[i] += res->level_hist[i]; }
+	else if (FILENAMEONLY && !counting) num_of_matched += res->n_matched ? 1 : 0;   /* the scan stops at the first hit (bitap.c:184-210, sgrep.c:813-814) */
+	else if (count_only) num_of_matched += (int)res->n_matched;
+	else {
+		for (i = 0; i < res->n_records; i++) print_record(hb, d, &recs[i], fname ? fname : "");
+	}
+	if (!counting) {
+		if (COUNT && !FILENAMEONLY) { if (FNAME) printf("%s: %d\n", fname, num_of_matched - before); else printf("%d\n", num_of_matched - before); }   /* agrep.c:3501-3557 */
+		if (FILENAMEONLY && num_of_matched > before) printf("%s\n", fname ? fname : "(standard input)");
+	}
+}
+
+static int scan_want(int counting, const unsigned long long *hist)
+{
+	const int count_only = counting || COUNT || SILENT || FILENAMEONLY;
+	/* output() needs j even without -n (agrep.c:3815) */
+	return count_only ? (hist ? AGB_WANT_LEVELS : AGB_WANT_COUNT) : (AGB_WANT_RECORDS | AGB_WANT_ORDINALS);
+}
+
+static agb_record *grow_list(agb_record *recs, size_t cap)
+{
+	if (cap) { recs = (agb_record *)realloc(recs, cap * sizeof *recs); if (!recs) { fprintf(stderr, "%s: out of memory\n", prog); exit(255); } }
+	return recs;
+}
+
+/* Files of up to SET_BYTES are gathered, in order, into sets of up to SET_BYTES and scanned by one agb_scan_set each: a small
+ * file alone costs a whole scan's fixed cost (copies, launches, a read-back), in a set it costs its bytes.  A larger file, and
+ * standard input, is scanned alone (agb_scan_host: stages 1 and 1.5 filter it, windows if it does not fit). */
+#define SET_BYTES (16u << 20)
+struct pending { const char *fname; unsigned char *hb; size_t n; };
+
+static void scan_set_of(const agb_pattern *p, struct pending *set, int nset, int counting, unsigned long long *hist)
+{
+	const agb_desc *d = agb_pattern_desc(p);
+	static const void *texts[4096]; static uint64_t sizes[4096]; static agb_result per[4096]; agb_result total;
+	agb_record *recs = NULL; size_t cap = 0, bytes = 0, at = 0; int i, rc;
+	const int want = scan_want(counting, hist);
+	for (i = 0; i < nset; i++) { texts[i] = set[i].hb + 1; sizes[i] = set[i].n; bytes += set[i].n; }
+	/* the list is sized from a guess; a set that reports more matching records than fit is scanned again with exactly
+	 * n_matched entries */
+	cap = (want & AGB_WANT_RECORDS) ? bytes / 64 + 65536 : 0;
+	for (;;) {
+		recs = grow_list(recs, cap);
+		rc = agb_scan_set(p, texts, sizes, (uint32_t)nset, want, recs, cap, per, &total);
+		if (rc) { fprintf(stderr, "%s: scan failed: %s\n", prog, agb_last_error()); exit(255); }   /* no CPU fallback */
+		if (!total.truncated) break;
+		cap = (size_t)total.n_matched;
+	}
+	for (i = 0; i < nset; i++) {
+		finish_file(d, set[i].fname, set[i].hb, &per[i], recs + at, counting, hist);
+		at += per[i].n_records;
+		free(set[i].hb);
+	}
+	free(recs);
+}
+
 /* one pass of exec() over the files (agrep.c:3411-3576); counting = the COUNT=ON passes of the -B sweep; hist (counting
  * only): a levels pass -- every file's histogram of smallest levels is added to hist[] */
 static int scan_files(const agb_pattern *p, char **files, int nfiles, int counting, unsigned long long *hist)
 {
-	int fi;
+	struct pending set[4096]; int nset = 0, fi; size_t set_bytes = 0;
+	const agb_desc *d = agb_pattern_desc(p);
 	for (fi = 0; fi < (nfiles ? nfiles : 1); fi++) {
 		const char *fname = nfiles ? files[fi] : NULL;
-		const agb_desc *d = agb_pattern_desc(p);
-		size_t n = 0, cap, i; unsigned char *hb = slurp(fname, &n, d->L, d->delim);
-		agb_result res; agb_record *recs = NULL; int before = num_of_matched, rc;
-		const int count_only = counting || COUNT || SILENT || FILENAMEONLY;
-		if (!hb) continue;
-		/* the list is sized from a guess; a scan that reports more matching records than fit (an empty record is a record:
-		 * -v on blank lines) is run again with exactly n_matched entries */
-		cap = count_only ? 0 : n / 64 + 65536;
+		size_t n = 0, cap; int unopened; unsigned char *hb = slurp(fname, &n, d->L, d->delim, &unopened);
+		agb_result res; agb_record *recs = NULL; int rc;
+		if (!hb) {
+			/* the files gathered before this one print first: messages and output keep the order of the files */
+			if (unopened) { if (nset) { scan_set_of(p, set, nset, counting, hist); nset = 0; set_bytes = 0; } cannot_open(fname); }
+			continue;
+		}
+		if (fname && n <= SET_BYTES) {
+			if (nset == 4096 || set_bytes + n > SET_BYTES) { scan_set_of(p, set, nset, counting, hist); nset = 0; set_bytes = 0; }
+			set[nset].fname = fname; set[nset].hb = hb; set[nset].n = n; nset++; set_bytes += n;
+			continue;
+		}
+		if (nset) { scan_set_of(p, set, nset, counting, hist); nset = 0; set_bytes = 0; }
+		cap = (scan_want(counting, hist) & AGB_WANT_RECORDS) ? n / 64 + 65536 : 0;
 		for (;;) {
-			if (cap) { recs = (agb_record *)realloc(recs, cap * sizeof *recs); if (!recs) { fprintf(stderr, "%s: out of memory\n", prog); exit(255); } }
-			rc = agb_scan_host(p, hb + 1, n, count_only ? (hist ? AGB_WANT_LEVELS : AGB_WANT_COUNT) : (AGB_WANT_RECORDS | AGB_WANT_ORDINALS)   /* output() needs j even without -n (agrep.c:3815) */, recs, cap, &res);
+			recs = grow_list(recs, cap);
+			rc = agb_scan_host(p, hb + 1, n, scan_want(counting, hist), recs, cap, &res);
 			if (rc) { fprintf(stderr, "%s: scan failed: %s\n", prog, agb_last_error()); exit(255); }   /* no CPU fallback */
 			if (!res.truncated) break;
 			cap = (size_t)res.n_matched;
 		}
-		if (hist) { for (i = 0; i <= AGB_MAXERR; i++) hist[i] += res.level_hist[i]; }
-		else if (FILENAMEONLY && !counting) num_of_matched += res.n_matched ? 1 : 0;   /* the scan stops at the first hit (bitap.c:184-210, sgrep.c:813-814) */
-		else if (count_only) num_of_matched += (int)res.n_matched;
-		else {
-			for (i = 0; i < res.n_records; i++) print_record(hb, d, &recs[i], fname ? fname : "");
-		}
-		if (!counting) {
-			if (COUNT && !FILENAMEONLY) { if (FNAME) printf("%s: %d\n", fname, num_of_matched - before); else printf("%d\n", num_of_matched - before); }   /* agrep.c:3501-3557 */
-			if (FILENAMEONLY && num_of_matched > before) printf("%s\n", fname ? fname : "(standard input)");
-		}
+		finish_file(d, fname, hb, &res, recs, counting, hist);
 		free(recs); free(hb);
 	}
+	if (nset) scan_set_of(p, set, nset, counting, hist);
 	return num_of_matched;
 }
 
@@ -156,7 +226,7 @@ static int regex_best_level(const char *pattern, agb_options *o, char **files, i
 	for (l = 0; l < passes; l++)
 		for (fi = 0; fi < nfiles; fi++) {
 			int fd = open(files[fi], O_RDONLY);
-			if (fd < 0) fprintf(stderr, "%s: can't open file for reading: %s\n", prog, files[fi]); else close(fd);
+			if (fd < 0) cannot_open(files[fi]); else close(fd);
 		}
 	if (best < 0 && !failed && lim > 4) fprintf(stderr, "%s: no match within 4 errors, the most a regular expression allows\n", prog);
 	num_of_matched = best > 0 ? (int)hist[best] : 0;

@@ -302,11 +302,17 @@ __device__ __forceinline__ uint32_t ord_count_seq(Reader &R, const OrdParams &P,
 	return cnt;
 }
 
-__global__ void __launch_bounds__(ORD_THREADS) k_delim_count(const OrdParams P)
+/* SET: block b counts tile set_tiles[b].tile of [0, n + L) of file set_tiles[b].file, and adds its count to the file's closes */
+template <bool SET = false>
+__global__ void __launch_bounds__(ORD_THREADS)
+k_delim_count(const OrdParams P0, const SetFile *set_files = nullptr, const SetTile *set_tiles = nullptr, unsigned long long *set_stats = nullptr)
 {
+	OrdParams Ps; uint64_t tile_ = 0; uint32_t file = 0;
+	if constexpr (SET) { Ps = P0; set_enter(set_files, set_tiles, Ps.text, Ps.n, tile_, file); }
+	const OrdParams &P = SET ? Ps : P0;
 	__shared__ uint32_t s_warp[ORD_THREADS / 32];
 	const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-	const int64_t n = (int64_t)P.n, limit = n + P.L, tile0 = (int64_t)blockIdx.x * ORD_TILE;
+	const int64_t n = (int64_t)P.n, limit = n + P.L, tile0 = (int64_t)(SET ? (unsigned)tile_ : blockIdx.x) * ORD_TILE;
 	uint32_t cnt = 0;                                           /* this thread's share of the tile */
 	if (P.L == 1 && tile0 + ORD_TILE <= n) {
 		/* a warp takes a 512-byte block per iteration, 16 bytes per lane (coalesced): exact per-byte equality by
@@ -341,7 +347,10 @@ __global__ void __launch_bounds__(ORD_THREADS) k_delim_count(const OrdParams P)
 	const uint32_t w = __reduce_add_sync(0xffffffffu, cnt);
 	if (lane == 0) s_warp[wid] = w;
 	__syncthreads();
-	if (tid == 0) { uint32_t t = 0; for (int i = 0; i < ORD_THREADS / 32; i++) t += s_warp[i]; P.tiles[blockIdx.x] = t; }
+	if (tid == 0) {
+		uint32_t t = 0; for (int i = 0; i < ORD_THREADS / 32; i++) t += s_warp[i]; P.tiles[blockIdx.x] = t;
+		if (SET && t) atomicAdd(&set_stats[SET_STATS * file + 10], (unsigned long long)t);
+	}
 }
 
 /* the tile counts from block counts that stage 1 already took (front.cu, COUNT): 64 blocks per tile, plus the
@@ -400,6 +409,27 @@ __global__ void __launch_bounds__(256) k_ordinals(const OrdParams P)
 	/* the virtual '\n' closes a record of its own when it completes a delimiter: only a 1-byte '\n' can */
 	const long long virt = (P.L == 1 && P.delim[0] == '\n') ? 1 : 0;
 	P.records[i].ordinal = (long long)j + virt + P.j0;
+}
+
+/* the ordinals of a set's list: a record's file is in its pad field; its j counts the delimiter ends of its own file, from
+ * the file's first ordinals tile (tile and block numbers below are the set's) */
+__global__ void __launch_bounds__(256) k_ordinals_set(const OrdParams P0, const SetFile *set_files)
+{
+	unsigned long long nrec = P0.totals[0];
+	if (nrec > P0.capacity) nrec = P0.capacity;
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= nrec) return;
+	const SetFile f = set_files[P0.records[i].pad];
+	OrdParams P = P0; P.text += f.off; P.n = f.n;
+	const int64_t q = P.records[i].end + P.L - 1;                          /* the last byte of the closing delimiter, in the file */
+	const uint64_t tile = f.ord_tile0 + (uint64_t)q / ORD_TILE, blk = (uint64_t)q / ORD_BLOCK;
+	const uint64_t b0 = tile * (ORD_TILE / ORD_BLOCK);
+	unsigned long long j = P.tile_off[tile] - P.tile_off[f.ord_tile0];
+	for (uint64_t b = b0; b < b0 + (uint64_t)(q % ORD_TILE) / ORD_BLOCK; b++) j += P.blocks[b];
+	if (P.L == 1) j += ord_count_swar(P, (int64_t)(blk * ORD_BLOCK), q + 1);
+	else { Reader R; R.init(P.text, P.n, P.delim, P.L); j += ord_count_seq(R, P, (int64_t)(blk * ORD_BLOCK), q + 1); }
+	const long long virt = (P.L == 1 && P.delim[0] == '\n') ? 1 : 0;
+	P.records[i].ordinal = (long long)j + virt + f.j0;
 }
 
 /* after stage 1: is the bitmap so full that thinning it (stage 1.5) and walking a candidate list cannot pay?  Then the
@@ -477,3 +507,27 @@ int ordinals_launch(const agb_desc &d, Workspace &W, const void *d_text, uint64_
 	return AGB_OK;
 }
 
+
+/* a set of files: the delimiter ends of every ordinals tile of every file (one launch), their scan over the whole set, the
+ * ordinals of the list.  d_ord_tiles: ceil((n + L) / ORD_TILE) tiles per file, file after file */
+int ordinals_set_launch(const agb_desc &d, Workspace &W, const void *d_text, const SetFile *d_files, const SetTile *d_ord_tiles,
+                        uint64_t ord_tiles, unsigned long long *d_stats, agb_record *d_records, uint64_t capacity, cudaStream_t st)
+{
+	if (ord_tiles + 1 > W.tiles) return AGB_ERR_NOMEM;
+	const size_t nb = (size_t)ord_tiles * (ORD_TILE / ORD_BLOCK);
+	if (nb > W.ord_blocks_cap) {
+		if (W.ord_blocks) cudaFree(W.ord_blocks);
+		W.ord_blocks = nullptr; W.ord_blocks_cap = 0;
+		CUDA_TRY(cudaMalloc(&W.ord_blocks, nb * sizeof(uint16_t))); W.ord_blocks_cap = nb;
+	}
+	OrdParams P; memset(&P, 0, sizeof P);
+	P.text = (const uint8_t *)d_text; P.blocks = W.ord_blocks; P.tiles = W.tile_counts; P.tile_off = W.tile_offsets;
+	P.records = d_records; P.totals = W.totals; P.capacity = capacity;
+	for (int i = 0; i < AGB_MAXDELIM + 2; i++) { P.dfold[i] = d.delim_fold[i]; P.delim[i] = d.delim[i] | d.delim_fold[i]; }
+	P.L = d.L; P.kind = d.delim_kind;
+	k_delim_count<true><<<(unsigned)ord_tiles, ORD_THREADS, 0, st>>>(P, d_files, d_ord_tiles, d_stats); g_launches++;
+	k_scan_tiles<<<1, 1024, 0, st>>>(W.tile_counts, W.tile_offsets, ord_tiles, nullptr); g_launches++;
+	if (d_records && capacity) { k_ordinals_set<<<(unsigned)((capacity + 255) / 256), 256, 0, st>>>(P, d_files); g_launches++; }
+	CUDA_TRY(cudaGetLastError());
+	return AGB_OK;
+}

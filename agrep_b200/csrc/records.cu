@@ -152,16 +152,20 @@ k_records(const RecParams P)
  * lockstep, bytes and the Mask[] table come from shared memory (global memory only for a record that outruns the
  * staged bytes), and nothing is carried between threads or tiles.  Same loop as asearch.c:94-199. */
 
-template <typename T, int NR, bool COSTS>
+template <typename T, int NR, bool COSTS, bool SET = false>
 __global__ void __launch_bounds__(DENSE_THREADS)
-k_records_dense(const RecParams P)
+k_records_dense(const RecParams P0)
 {
+	/* SET: this block's tile of a file of the set, the file's text as the whole text */
+	RecParams Ps; uint64_t tile = blockIdx.x; uint32_t file = 0;
+	if constexpr (SET) { Ps = P0; set_enter(P0.set_files, P0.set_tiles, Ps.text, Ps.n, tile, file); Ps.n_chunks = (Ps.n + 15) / 16; }
+	const RecParams &P = SET ? Ps : P0;
 	extern __shared__ __align__(128) uint8_t s_text[];                 /* DENSE_TILE + DENSE_TAIL */
 	__shared__ RecShared<T, NR> SH;
 	__shared__ uint64_t s_bar;
 	__shared__ uint32_t s_scan[DENSE_THREADS];
 	const uint32_t tid = threadIdx.x;
-	const int64_t n = (int64_t)P.n, tile0 = (int64_t)blockIdx.x * DENSE_TILE;
+	const int64_t n = (int64_t)P.n, tile0 = (int64_t)tile * DENSE_TILE;
 	const uint64_t readable = P.n_chunks * 16;
 	const uint64_t avail = (readable - (uint64_t)tile0) & ~15ull;
 	const uint32_t loaded = (uint32_t)(avail < (uint64_t)(DENSE_TILE + DENSE_TAIL) ? avail : (uint64_t)(DENSE_TILE + DENSE_TAIL));
@@ -288,7 +292,7 @@ k_records_dense(const RecParams P)
 							const uint64_t at = out_pos + cnt;
 							if (at < P.capacity) {
 								agb_record rec; rec.begin = tile0 + (int64_t)(int32_t)begin_rel; rec.end = tile0 + end_rel;
-								rec.ordinal = 0; rec.level = level; rec.pad = 0;
+								rec.ordinal = 0; rec.level = level; rec.pad = (int32_t)file;
 								P.records[at] = rec;
 							}
 						}
@@ -322,7 +326,7 @@ k_records_dense(const RecParams P)
 							if (pass == 1) {
 								const uint64_t at = out_pos + cnt;
 								if (at < P.capacity) {
-									agb_record rec; rec.begin = begin; rec.end = end; rec.ordinal = 0; rec.level = level; rec.pad = 0;
+									agb_record rec; rec.begin = begin; rec.end = end; rec.ordinal = 0; rec.level = level; rec.pad = (int32_t)file;
 									P.records[at] = rec;
 								}
 							}
@@ -350,10 +354,12 @@ k_records_dense(const RecParams P)
 				if (tid == DENSE_THREADS - 1) {
 					P.tile_counts[blockIdx.x] = s_scan[DENSE_THREADS - 1];
 					if (s_scan[DENSE_THREADS - 1]) atomicAdd(&P.totals[0], (unsigned long long)s_scan[DENSE_THREADS - 1]);
+					if (SET && s_scan[DENSE_THREADS - 1]) atomicAdd(&P.set_stats[SET_STATS * file], (unsigned long long)s_scan[DENSE_THREADS - 1]);
 					atomicAdd(&P.totals[1], (unsigned long long)((tile_len + 15) / 16));
 				}
 				__syncthreads();
 				if (P.levels && tid <= AGB_MAXERR && SH.hist[tid]) atomicAdd(&P.totals[2 + tid], SH.hist[tid]);
+				if (SET && P.levels && tid <= AGB_MAXERR && SH.hist[tid]) atomicAdd(&P.set_stats[SET_STATS * file + 1 + tid], SH.hist[tid]);
 			} else out_pos = P.tile_offsets[blockIdx.x] + (s_scan[tid] - my_count);
 		}
 	}
@@ -455,41 +461,44 @@ int launch_records(const agb_desc &d, const RecParams &P, unsigned grid, cudaStr
 	return narrow ? launch_records_t<uint32_t, false>(d.nrows, P, grid, st) : launch_records_t<uint64_t, false>(d.nrows, P, grid, st);
 }
 
-template <typename T, int NR, bool COSTS>
+template <typename T, int NR, bool COSTS, bool SET>
 static void launch_dense_one(const RecParams &P, unsigned grid, cudaStream_t st)
 {
 	static bool configured[64] = {false};
 	int dev = 0; cudaGetDevice(&dev);
 	if (!configured[dev & 63]) {
-		cudaFuncSetAttribute(k_records_dense<T, NR, COSTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, DENSE_SMEM);
+		cudaFuncSetAttribute(k_records_dense<T, NR, COSTS, SET>, cudaFuncAttributeMaxDynamicSharedMemorySize, DENSE_SMEM);
 		configured[dev & 63] = true;
 	}
-	k_records_dense<T, NR, COSTS><<<grid, DENSE_THREADS, DENSE_SMEM, st>>>(P);
+	k_records_dense<T, NR, COSTS, SET><<<grid, DENSE_THREADS, DENSE_SMEM, st>>>(P);
 }
-template <typename T, bool COSTS>
+template <typename T, bool COSTS, bool SET>
 static int launch_dense_t(int nrows, const RecParams &P, unsigned grid, cudaStream_t st)
 {
 	switch (nrows) {
-	case 1: launch_dense_one<T, 1, COSTS>(P, grid, st); break;
-	case 2: launch_dense_one<T, 2, COSTS>(P, grid, st); break;
-	case 3: launch_dense_one<T, 3, COSTS>(P, grid, st); break;
-	case 4: launch_dense_one<T, 4, COSTS>(P, grid, st); break;
-	case 5: launch_dense_one<T, 5, COSTS>(P, grid, st); break;
-	case 6: launch_dense_one<T, 6, COSTS>(P, grid, st); break;
-	case 7: launch_dense_one<T, 7, COSTS>(P, grid, st); break;
-	case 8: launch_dense_one<T, 8, COSTS>(P, grid, st); break;
-	case 9: launch_dense_one<T, 9, COSTS>(P, grid, st); break;
+	case 1: launch_dense_one<T, 1, COSTS, SET>(P, grid, st); break;
+	case 2: launch_dense_one<T, 2, COSTS, SET>(P, grid, st); break;
+	case 3: launch_dense_one<T, 3, COSTS, SET>(P, grid, st); break;
+	case 4: launch_dense_one<T, 4, COSTS, SET>(P, grid, st); break;
+	case 5: launch_dense_one<T, 5, COSTS, SET>(P, grid, st); break;
+	case 6: launch_dense_one<T, 6, COSTS, SET>(P, grid, st); break;
+	case 7: launch_dense_one<T, 7, COSTS, SET>(P, grid, st); break;
+	case 8: launch_dense_one<T, 8, COSTS, SET>(P, grid, st); break;
+	case 9: launch_dense_one<T, 9, COSTS, SET>(P, grid, st); break;
 	default: return -1;
 	}
 	g_launches++;
 	return 0;
 }
-int launch_dense(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st)
+template <bool SET>
+static int launch_dense_any(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st)
 {
 	const bool costs = d.engine == AGB_ENGINE_ASEARCH1, narrow = d.M <= 31;
-	if (costs) return narrow ? launch_dense_t<uint32_t, true>(d.nrows, P, grid, st) : launch_dense_t<uint64_t, true>(d.nrows, P, grid, st);
-	return narrow ? launch_dense_t<uint32_t, false>(d.nrows, P, grid, st) : launch_dense_t<uint64_t, false>(d.nrows, P, grid, st);
+	if (costs) return narrow ? launch_dense_t<uint32_t, true, SET>(d.nrows, P, grid, st) : launch_dense_t<uint64_t, true, SET>(d.nrows, P, grid, st);
+	return narrow ? launch_dense_t<uint32_t, false, SET>(d.nrows, P, grid, st) : launch_dense_t<uint64_t, false, SET>(d.nrows, P, grid, st);
 }
+int launch_dense(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st) { return launch_dense_any<false>(d, P, grid, st); }
+int launch_dense_set(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st) { return launch_dense_any<true>(d, P, grid, st); }
 
 template <typename T, bool COSTS>
 static int launch_records_list_t(int nrows, const RecParams &P, unsigned grid, cudaStream_t st)

@@ -25,7 +25,6 @@
 #include "automaton.cuh"
 
 #define RX_THREADS 256
-#define RX_TILE    32768
 #define RX_TAIL    2048
 #define RX_PER     (RX_TILE / RX_THREADS)          /* 128 bytes per thread */
 static_assert(RX_TILE == DENSE_TILE, "the tile counts of the workspace are sized for DENSE_TILE");
@@ -63,10 +62,14 @@ __device__ __forceinline__ bool rx_line_matches(T s, const T *tab, T mask_nl, T 
 	return ((t & (T)1) != 0) != inverse;
 }
 
-template <typename T, int NR, bool LEVELS>
+template <typename T, int NR, bool LEVELS, bool SET = false>
 __global__ void __launch_bounds__(RX_THREADS)
-k_regex(const RecParams P)
+k_regex(const RecParams P0)
 {
+	/* SET: this block's tile of a file of the set, the file's text as the whole text */
+	RecParams Ps; uint64_t tile = 0; uint32_t file = 0;
+	if constexpr (SET) { Ps = P0; set_enter(P0.set_files, P0.set_tiles, Ps.text, Ps.n, tile, file); Ps.n_chunks = (Ps.n + 15) / 16; }
+	const RecParams &P = SET ? Ps : P0;
 	extern __shared__ __align__(16) uint8_t s_raw[];
 	T *s_tab = reinterpret_cast<T *>(s_raw);                               /* sizeof(T) slices of 256 */
 	T *s_mask = s_tab + sizeof(T) * 256;                                   /* 256 */
@@ -78,7 +81,7 @@ k_regex(const RecParams P)
 	const T *g_tab = reinterpret_cast<const T *>(P.rx_tab);
 	for (uint32_t i = tid; i < sizeof(T) * 256; i += RX_THREADS) s_tab[i] = g_tab[i];
 	for (uint32_t i = tid; i < 256; i += RX_THREADS) s_mask[i] = (T)D->mask[i];
-	const int64_t n = (int64_t)P.n, tile0 = (int64_t)blockIdx.x * RX_TILE;
+	const int64_t n = (int64_t)P.n, tile0 = (int64_t)(SET ? (unsigned)tile : blockIdx.x) * RX_TILE;
 	const uint64_t readable = P.n_chunks * 16;
 	const uint64_t avail = (readable - (uint64_t)tile0) & ~15ull;
 	const uint32_t loaded = (uint32_t)(avail < (uint64_t)(RX_TILE + RX_TAIL) ? avail : (uint64_t)(RX_TILE + RX_TAIL));
@@ -170,7 +173,7 @@ k_regex(const RecParams P)
 					if (pass == 1) {
 						const uint64_t at = out_pos + cnt;
 						if (at < P.capacity) {
-							agb_record rec; rec.begin = begin; rec.end = p; rec.ordinal = 0; rec.level = LEVELS ? level : D->k; rec.pad = 0;
+							agb_record rec; rec.begin = begin; rec.end = p; rec.ordinal = 0; rec.level = LEVELS ? level : D->k; rec.pad = (int32_t)file;
 							P.records[at] = rec;
 						}
 					}
@@ -196,9 +199,11 @@ k_regex(const RecParams P)
 				if (tid == RX_THREADS - 1) {
 					P.tile_counts[blockIdx.x] = s_scan[RX_THREADS - 1];
 					if (s_scan[RX_THREADS - 1]) atomicAdd(&P.totals[0], (unsigned long long)s_scan[RX_THREADS - 1]);
+					if (SET && s_scan[RX_THREADS - 1]) atomicAdd(&P.set_stats[SET_STATS * file], (unsigned long long)s_scan[RX_THREADS - 1]);
 					atomicAdd(&P.totals[1], (unsigned long long)((tile_len + 15) / 16));
 				}
 				if (LEVELS && tid < NR && s_hist[tid]) atomicAdd(&P.totals[2 + tid], (unsigned long long)s_hist[tid]);
+				if (SET && LEVELS && tid < NR && s_hist[tid]) atomicAdd(&P.set_stats[SET_STATS * file + 1 + tid], (unsigned long long)s_hist[tid]);
 			} else out_pos = P.tile_offsets[blockIdx.x] + (s_scan[tid] - my_count);
 		}
 	}
@@ -206,27 +211,27 @@ k_regex(const RecParams P)
 
 template <typename T> static constexpr size_t rx_smem() { return sizeof(T) * 256 * sizeof(T) + 256 * sizeof(T) + RX_TILE + RX_TAIL; }
 
-template <typename T, int NR, bool LEVELS>
+template <typename T, int NR, bool LEVELS, bool SET>
 static void launch_regex_one(const RecParams &P, unsigned grid, cudaStream_t st)
 {
 	static bool configured[64] = {false};
 	int dev = 0; cudaGetDevice(&dev);
 	if (!configured[dev & 63]) {
-		cudaFuncSetAttribute(k_regex<T, NR, LEVELS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rx_smem<T>());
+		cudaFuncSetAttribute(k_regex<T, NR, LEVELS, SET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rx_smem<T>());
 		configured[dev & 63] = true;
 	}
-	k_regex<T, NR, LEVELS><<<grid, RX_THREADS, rx_smem<T>(), st>>>(P);
+	k_regex<T, NR, LEVELS, SET><<<grid, RX_THREADS, rx_smem<T>(), st>>>(P);
 }
 
-template <typename T, bool LEVELS>
+template <typename T, bool LEVELS, bool SET>
 static int launch_regex_t(int nrows, const RecParams &P, unsigned grid, cudaStream_t st)
 {
 	switch (nrows) {
-	case 1: launch_regex_one<T, 1, LEVELS>(P, grid, st); break;
-	case 2: launch_regex_one<T, 2, LEVELS>(P, grid, st); break;
-	case 3: launch_regex_one<T, 3, LEVELS>(P, grid, st); break;
-	case 4: launch_regex_one<T, 4, LEVELS>(P, grid, st); break;
-	case 5: launch_regex_one<T, 5, LEVELS>(P, grid, st); break;
+	case 1: launch_regex_one<T, 1, LEVELS, SET>(P, grid, st); break;
+	case 2: launch_regex_one<T, 2, LEVELS, SET>(P, grid, st); break;
+	case 3: launch_regex_one<T, 3, LEVELS, SET>(P, grid, st); break;
+	case 4: launch_regex_one<T, 4, LEVELS, SET>(P, grid, st); break;
+	case 5: launch_regex_one<T, 5, LEVELS, SET>(P, grid, st); break;
 	default: return -1;
 	}
 	g_launches++;
@@ -236,13 +241,16 @@ static int launch_regex_t(int nrows, const RecParams &P, unsigned grid, cudaStre
 /* 32-bit words hold positions 0..31 (M <= 31), 64-bit words the rest */
 bool regex_narrow(const agb_desc &d) { return d.M <= 31; }
 
-int launch_regex(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st)
+template <bool SET>
+static int launch_regex_any(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st)
 {
 	if (!P.rx_tab) return -1;
 	if (P.levels)
-		return regex_narrow(d) ? launch_regex_t<uint32_t, true>(d.nrows, P, grid, st) : launch_regex_t<uint64_t, true>(d.nrows, P, grid, st);
-	return regex_narrow(d) ? launch_regex_t<uint32_t, false>(d.nrows, P, grid, st) : launch_regex_t<uint64_t, false>(d.nrows, P, grid, st);
+		return regex_narrow(d) ? launch_regex_t<uint32_t, true, SET>(d.nrows, P, grid, st) : launch_regex_t<uint64_t, true, SET>(d.nrows, P, grid, st);
+	return regex_narrow(d) ? launch_regex_t<uint32_t, false, SET>(d.nrows, P, grid, st) : launch_regex_t<uint64_t, false, SET>(d.nrows, P, grid, st);
 }
+int launch_regex(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st) { return launch_regex_any<false>(d, P, grid, st); }
+int launch_regex_set(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st) { return launch_regex_any<true>(d, P, grid, st); }
 
 /* the byte-sliced Next tables of a regular expression, in the word width the kernel uses: slice s, byte value v ->
  * the union of follow[p] over the positions p whose bit (M - p) is bit i of v at 8 s + i */

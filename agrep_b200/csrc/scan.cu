@@ -26,6 +26,7 @@
 #include <memory>
 #include <mutex>
 #include <thread>
+#include <vector>
 
 /* ------------------------------------------------------------------------------------------------ */
 thread_local char g_err[512];
@@ -632,6 +633,8 @@ struct SliceSource {
 	off_t fd_off = 0;              /* where the text starts in it (-1: lseek failed, and n is 0) */
 	int dfd = -1;                  /* the same file opened with O_DIRECT, or -1; closed for good when a read through it fails */
 	uint64_t n = 0;
+	/* a set of texts (agb_scan_set): text i is bytes [part_at[i], part_at[i] + part_n[i]) of the source, zeros in between */
+	const void *const *parts = nullptr; const uint64_t *part_at = nullptr, *part_n = nullptr; uint32_t n_parts = 0;
 	SliceSource(const void *h_text = nullptr, uint64_t len = 0) : mem((const uint8_t *)h_text), n(len)
 	{
 		cudaPointerAttributes attr; memset(&attr, 0, sizeof attr);
@@ -654,6 +657,20 @@ static bool fd_source(int fd, SliceSource &src)
 	return true;
 }
 
+/* bytes [off, off + len) of a set's source (SliceSource.parts) into dst */
+static void gather_slice(const SliceSource &src, uint64_t off, uint8_t *dst, size_t len)
+{
+	const uint64_t end = off + len;
+	uint64_t p = off;
+	uint32_t i = (uint32_t)(std::upper_bound(src.part_at, src.part_at + src.n_parts, off) - src.part_at);
+	for (i = i ? i - 1 : 0; p < end && i < src.n_parts; i++) {
+		const uint64_t a = src.part_at[i], b = a + src.part_n[i];
+		if (p < a) { const uint64_t z = std::min(a, end) - p; memset(dst + (p - off), 0, z); p += z; }
+		if (p < end && p < b) { const uint64_t c = std::min(b, end) - p; memcpy(dst + (p - off), (const uint8_t *)src.parts[i] + (p - a), c); p += c; }
+	}
+	if (p < end) memset(dst + (p - off), 0, end - p);
+}
+
 /* bytes [off, off + len) of a pageable or file source into the ring buffer dst: 4 host threads memcpy or pread(2) a quarter
  * each (one thread's memcpy, or read(2) from the page cache, is a third of what PCIe takes; under 1 MiB of memory one thread
  * does).  Through the O_DIRECT descriptor whole 4 KiB blocks are asked for (the ring's buffers are page aligned and a multiple
@@ -661,6 +678,7 @@ static bool fd_source(int fd, SliceSource &src)
 static bool fill_slice(SliceSource &src, uint64_t off, uint8_t *dst, size_t len)
 {
 	if (src.mem && len < (1u << 20)) { memcpy(dst, src.mem + off, len); return true; }
+	if (src.parts && len < (1u << 20)) { gather_slice(src, off, dst, len); return true; }
 	for (;;) {
 		const bool direct = !src.mem && src.dfd >= 0;
 		const int fd = direct ? src.dfd : src.fd, T = 4;
@@ -671,7 +689,8 @@ static bool fill_slice(SliceSource &src, uint64_t off, uint8_t *dst, size_t len)
 			const size_t l = std::min(part, len - a);
 			const uint8_t *mem = src.mem ? src.mem + off + a : nullptr;
 			const off_t at = src.fd_off + (off_t)(off + a);
-			th[used++] = std::thread([=, &bad] {
+			th[used++] = std::thread([=, &src, &bad] {
+				if (src.parts) { gather_slice(src, off + a, dst + a, l); return; }
 				if (mem) { memcpy(dst + a, mem, l); return; }
 				for (size_t got = 0; got < l; ) {
 					const size_t ask = direct ? ((l - got + 4095) & ~(size_t)4095) : l - got;
@@ -696,6 +715,7 @@ struct HostPath {
 	uint8_t *ring[STAGE_BUFS] = {nullptr, nullptr, nullptr};
 	uint8_t *text = nullptr; size_t text_cap = 0;          /* (capacities in bytes) */
 	agb_record *rec = nullptr; size_t rec_cap = 0;
+	uint8_t *set_meta = nullptr; size_t set_meta_cap = 0;  /* agb_scan_set: its file and tile tables, the per-file counters */
 };
 static HostPath g_host[64];
 static std::mutex g_host_mu[64];
@@ -714,12 +734,12 @@ static void host_release(int dev)
 {
 	std::lock_guard<std::mutex> lk(g_host_mu[dev]);
 	HostPath &H = g_host[dev];
-	if (!H.s_copy && !H.text && !H.rec) return;              /* (the events and the ring are made after s_copy) */
+	if (!H.s_copy && !H.text && !H.rec && !H.set_meta) return;              /* (the events and the ring are made after s_copy) */
 	if (cudaSetDevice(dev) != cudaSuccess) { cudaGetLastError(); return; }
 	cudaDeviceSynchronize();
 	for (int i = 0; i < STAGE_BUFS; i++) { if (H.ev[i]) cudaEventDestroy(H.ev[i]); cudaFreeHost(H.ring[i]); }
 	if (H.s_copy) cudaStreamDestroy(H.s_copy); if (H.s_comp) cudaStreamDestroy(H.s_comp);
-	cudaFree(H.text); cudaFree(H.rec);
+	cudaFree(H.text); cudaFree(H.rec); cudaFree(H.set_meta);
 	H = HostPath();
 }
 
@@ -1033,6 +1053,146 @@ extern "C" int agb_scan_fd_windowed(const agb_pattern *p, int fd, uint64_t windo
 {
 	if (!window_ok(window_bytes)) return AGB_ERR_ARG;
 	return scan_fd_any(p, fd, window_bytes, want, records, capacity, res);
+}
+
+/* ------------------------------------------------------------------------------------------------
+ * a set of files in one pass (DESIGN 3.4.1).  `agrep pattern *.c` scans many small files; one agb_scan_host per file pays
+ * the fixed cost of a scan (copies, about ten launches, a synchronising read-back) per file.  Here the files go through the
+ * pinned ring into one device buffer, each at a 16-byte boundary, and one launch sequence scans them all: the record stage's
+ * tile form (k_records_dense, k_regex) and the ordinals in their SET form, one block per 32 KiB tile of a file, each block
+ * taking its file's bounds as the text's.  A file's records come out in one ordered list, file after file, offsets and
+ * ordinals relative to the file, the file's index in agb_record.pad; per-file counts are added up by the blocks.  Stages 1
+ * and 1.5 do not run: the tile form walks every byte, which on small files costs less than the launches and the read-back
+ * that the filters would add per file.
+ * ---------------------------------------------------------------------------------------------- */
+extern "C" int agb_scan_set(const agb_pattern *p, const void *const *h_texts, const uint64_t *sizes, uint32_t n_files, int want,
+                            agb_record *records, uint64_t capacity, agb_result *per_file, agb_result *total)
+{
+	if (!p || !total) return AGB_ERR_ARG;
+	memset(total, 0, sizeof *total);
+	if (!n_files) {
+		if (h_texts || sizes || per_file) { snprintf(g_err, sizeof g_err, "agb_scan_set: no files, but file arrays were given"); return AGB_ERR_ARG; }
+		return AGB_OK;
+	}
+	if (!h_texts || !sizes || !per_file) { snprintf(g_err, sizeof g_err, "agb_scan_set: h_texts, sizes and per_file are needed"); return AGB_ERR_ARG; }
+	const bool want_list = (want & AGB_WANT_RECORDS) && capacity, ord = (want & AGB_WANT_ORDINALS) != 0;
+	if (want_list && !records) { snprintf(g_err, sizeof g_err, "agb_scan_set: a capacity without a record list"); return AGB_ERR_ARG; }
+	for (uint32_t i = 0; i < n_files; i++)
+		if (!h_texts[i] && sizes[i]) { snprintf(g_err, sizeof g_err, "agb_scan_set: file %u has no text but %llu bytes", i, (unsigned long long)sizes[i]); return AGB_ERR_ARG; }
+	const agb_desc &d = p->d;
+	const agb_regex *rx = agb_pattern_regex(p);
+	/* the layout: file i at at[i]; its record tiles (of the kernel that runs) and its ordinals tiles (of [0, n + L)) */
+	const uint64_t rec_tile = d.engine == AGB_ENGINE_REGEX ? RX_TILE : DENSE_TILE;
+	std::vector<uint64_t> at(n_files);
+	std::vector<SetFile> files(n_files);
+	std::vector<SetTile> rtiles, otiles;
+	uint64_t bytes = 0;
+	for (uint32_t i = 0; i < n_files; i++) {
+		const uint64_t n = sizes[i];
+		at[i] = bytes;
+		files[i].off = bytes; files[i].n = n; files[i].ord_tile0 = (uint32_t)otiles.size();
+		/* bitap.c:151-156, as ordinals_launch */
+		files[i].j0 = (d.user_delim && d.engine != AGB_ENGINE_ASEARCH0 && n >= (uint64_t)d.L && memcmp(h_texts[i], d.delim, (size_t)d.L) == 0) ? -1 : 0;
+		for (uint64_t t = 0; t * rec_tile < n; t++) rtiles.push_back(SetTile{i, (uint32_t)t});
+		for (uint64_t t = 0; t * ORD_TILE < n + (uint64_t)d.L; t++) otiles.push_back(SetTile{i, (uint32_t)t});
+		bytes += (n + 15) & ~15ull;
+	}
+	int dev = 0; CUDA_TRY(cudaGetDevice(&dev));
+	if (dev < 0 || dev >= 64) return AGB_ERR_ARG;
+	std::lock_guard<std::mutex> hlk(g_host_mu[dev]);
+	std::lock_guard<std::mutex> lk(g_ws_mu[dev]);
+	HostPath &H = g_host[dev];
+	Workspace &W = g_ws[dev];
+	const size_t need = (size_t)bytes + 4096;
+	const uint64_t cap_bytes = max_text_bytes();
+	const cudaError_t e = (cap_bytes && need > cap_bytes) ? cudaErrorMemoryAllocation : dev_reserve(&H.text, &H.text_cap, need);
+	if (e == cudaErrorMemoryAllocation) {
+		snprintf(g_err, sizeof g_err, "a set of %u files (%llu bytes on the device) does not fit in device memory; scan it in smaller sets",
+		         n_files, (unsigned long long)need);
+		return AGB_ERR_NOMEM;
+	}
+	CUDA_TRY(e);
+	/* no record is shorter than a byte but the empty ones, at most one per byte and file: the list never needs more */
+	const uint64_t list_cap = want_list ? std::min<uint64_t>(capacity, bytes + 2ull * n_files) : 0;
+	static_assert(RX_TILE == DENSE_TILE && ORD_TILE == DENSE_TILE, "ws_prepare sizes the tile counts for DENSE_TILE");
+	int rc = ws_prepare(W, (uint64_t)std::max(rtiles.size(), otiles.size()) * DENSE_TILE); if (rc) return rc;
+	SliceSource src;
+	src.parts = h_texts; src.part_at = at.data(); src.part_n = sizes; src.n_parts = n_files; src.n = bytes;
+	rc = host_ensure(H, src); if (rc) return rc;
+	CUDA_TRY(dev_reserve(&H.rec, &H.rec_cap, list_cap * sizeof(agb_record)));
+	const size_t fb = files.size() * sizeof(SetFile), rb = rtiles.size() * sizeof(SetTile), ob = otiles.size() * sizeof(SetTile);
+	const size_t sb = (size_t)n_files * SET_STATS * sizeof(unsigned long long);
+	const size_t o_r = (fb + 15) & ~(size_t)15, o_o = o_r + ((rb + 15) & ~(size_t)15), o_s = o_o + ((ob + 15) & ~(size_t)15);
+	CUDA_TRY(dev_reserve(&H.set_meta, &H.set_meta_cap, o_s + sb));
+	SetFile *d_files = reinterpret_cast<SetFile *>(H.set_meta);
+	SetTile *d_rtiles = reinterpret_cast<SetTile *>(H.set_meta + o_r), *d_otiles = reinterpret_cast<SetTile *>(H.set_meta + o_o);
+	unsigned long long *d_stats = reinterpret_cast<unsigned long long *>(H.set_meta + o_s);
+	CUDA_TRY(cudaMemcpyAsync(d_files, files.data(), fb, cudaMemcpyHostToDevice, H.s_comp));
+	if (rb) CUDA_TRY(cudaMemcpyAsync(d_rtiles, rtiles.data(), rb, cudaMemcpyHostToDevice, H.s_comp));
+	CUDA_TRY(cudaMemcpyAsync(d_otiles, otiles.data(), ob, cudaMemcpyHostToDevice, H.s_comp));
+	CUDA_TRY(cudaMemsetAsync(d_stats, 0, sb, H.s_comp));
+	rc = ws_upload_desc(W, d, H.s_comp); if (rc) return rc;
+	rc = regex_prepare(W, d, rx, H.s_comp); if (rc) return rc;
+	CUDA_TRY(cudaMemsetAsync(W.totals, 0, 16 * sizeof(unsigned long long), H.s_comp));
+	rc = upload(H, src, 0, bytes, H.text, need - bytes, [&](uint64_t, cudaEvent_t ev) -> int {
+		CUDA_TRY(cudaStreamWaitEvent(H.s_comp, ev, 0));
+		return AGB_OK;
+	});
+	if (rc) return rc;
+	if (!bytes) CUDA_TRY(cudaStreamSynchronize(H.s_copy));     /* (the slack's zeroing: no slice event follows it) */
+	CUDA_TRY(cudaEventRecord(W.e1, H.s_comp));
+	RecParams P; memset(&P, 0, sizeof P);
+	P.text = H.text; P.n = bytes; P.desc = W.d_desc; P.records = H.rec; P.capacity = list_cap; P.totals = W.totals;
+	P.levels = (want & AGB_WANT_LEVELS) ? 1 : 0; P.want_level = -1;
+	P.own_lo = INT64_MIN; P.own_hi = INT64_MAX; P.shard_last = 1;
+	P.rx_tab = W.d_regex; P.rx_tail = W.regex_tail;
+	P.tile_counts = W.tile_counts; P.tile_offsets = W.tile_offsets;
+	P.set_files = d_files; P.set_tiles = d_rtiles; P.set_stats = d_stats;
+	const bool regex = d.engine == AGB_ENGINE_REGEX;
+	const unsigned grid = (unsigned)rtiles.size();
+	if (grid) {
+		if (regex ? launch_regex_set(d, P, grid, H.s_comp) : launch_dense_set(d, P, grid, H.s_comp)) return AGB_ERR_ARG;
+		CUDA_TRY(cudaGetLastError());
+		if (want_list) {
+			k_scan_tiles<<<1, 1024, 0, H.s_comp>>>(W.tile_counts, W.tile_offsets, grid, nullptr); g_launches++;
+			P.emit = 1;
+			if (regex ? launch_regex_set(d, P, grid, H.s_comp) : launch_dense_set(d, P, grid, H.s_comp)) return AGB_ERR_ARG;
+			CUDA_TRY(cudaGetLastError());
+		}
+	}
+	if (ord) { rc = ordinals_set_launch(d, W, H.text, d_files, d_otiles, otiles.size(), d_stats, want_list ? H.rec : nullptr, list_cap, H.s_comp); if (rc) return rc; }
+	CUDA_TRY(cudaEventRecord(W.e2, H.s_comp));
+	std::vector<unsigned long long> stats((size_t)n_files * SET_STATS);
+	CUDA_TRY(cudaMemcpyAsync(stats.data(), d_stats, sb, cudaMemcpyDeviceToHost, H.s_comp));
+	CUDA_TRY(cudaStreamSynchronize(H.s_comp));
+	const uint64_t virt = (d.L == 1 && d.delim[0] == '\n') ? 1 : 0;   /* the virtual '\n' closes a record of its own (ordinals_launch) */
+	for (uint32_t i = 0; i < n_files; i++) {
+		agb_result &r = per_file[i];
+		const unsigned long long *st = &stats[(size_t)i * SET_STATS];
+		memset(&r, 0, sizeof r);
+		r.n_matched = st[0];
+		for (int l = 0; l <= AGB_MAXERR; l++) r.level_hist[l] = st[1 + l];
+		r.n_closes = ord ? st[10] + virt : 0;
+		if (want & AGB_WANT_RECORDS) {
+			const uint64_t room = capacity > total->n_matched ? capacity - total->n_matched : 0;
+			r.n_records = std::min<uint64_t>(r.n_matched, room);
+			r.truncated = r.n_matched > room ? 1 : 0;
+		}
+		total->n_matched += r.n_matched;
+		for (int l = 0; l <= AGB_MAXERR; l++) total->level_hist[l] += r.level_hist[l];
+		total->n_closes += r.n_closes;
+	}
+	if (want & AGB_WANT_RECORDS) {
+		total->n_records = std::min<uint64_t>(total->n_matched, capacity);
+		total->truncated = total->n_matched > capacity ? 1 : 0;
+	}
+	if (total->n_records) {
+		CUDA_TRY(cudaMemcpyAsync(records, H.rec, total->n_records * sizeof(agb_record), cudaMemcpyDeviceToHost, H.s_comp));
+		CUDA_TRY(cudaStreamSynchronize(H.s_comp));
+	}
+	CUDA_TRY(cudaStreamSynchronize(H.s_copy));
+	CUDA_TRY(cudaEventElapsedTime(&total->ms_records, W.e1, W.e2));
+	return AGB_OK;
 }
 
 /* ---- a text kept in HBM across scans (the drop-in layer's exec() scans the same file K + 2 times under -B,

@@ -104,10 +104,21 @@ struct RecParams {
 	int64_t own_lo, own_hi; int shard_last;
 	/* regular expressions (regex.cu): the byte-sliced Next tables on the device, TAIL's epsilon move at '\n' */
 	const void *rx_tab; int rx_tail;
+	/* a set of files (agb_scan_set, the kernels' SET form): block b scans tile set_tiles[b].tile of file set_tiles[b].file */
+	const struct SetFile *set_files; const struct SetTile *set_tiles; unsigned long long *set_stats;
 };
+/* agb_scan_set: file f is the text [off, off + n) of one device buffer (off a multiple of 16), scanned as if alone.  A tile of
+ * the record stage (32 KiB) and of the ordinals (32 KiB of [0, n + L)) lies in one file, so a block of the SET form takes its
+ * file's text bounds where a whole-text scan takes 0 and n, and nothing is carried across a file's edge.  Per file, the
+ * blocks add into set_stats[SET_STATS f + ...]: [0] matching records, [1 + l] records of smallest level l, [10] record
+ * closes (ordinals).  j0: -1 when the file starts with the user's delimiter (bitap.c:151-156). */
+struct SetFile { uint64_t off, n; uint32_t ord_tile0; int32_t j0; };
+struct SetTile { uint32_t file, tile; };
+#define SET_STATS 16
 struct ShardInfo { int64_t own_lo, own_hi; int last; };
 #define DENSE_THREADS 256
 #define DENSE_TILE    32768
+#define RX_TILE       32768                               /* regex.cu: k_regex's tile */
 #define DENSE_TAIL    2048
 #define DENSE_PER     (DENSE_TILE / DENSE_THREADS)          /* 128 bytes per thread */
 #define DENSE_SMEM (DENSE_TILE + DENSE_TAIL)
@@ -200,6 +211,9 @@ int  compact_ranges_launch(Workspace &W, uint64_t n, cudaStream_t st);
 /* records.cu, slices.cu: one launch of the given form (count pass or emit pass, RecParams.emit) */
 int  launch_records(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 int  launch_dense(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
+/* the SET form of the dense tile kernel and of k_regex: one block per entry of P.set_tiles */
+int  launch_dense_set(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
+int  launch_regex_set(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 int  launch_records_list(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 int  launch_slices(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 bool slices_usable(const agb_desc &d);
@@ -218,4 +232,15 @@ __global__ void k_scan_apply(const uint32_t *counts, uint64_t n, const uint64_t 
 int  front_is_dense(Workspace &W, uint64_t n, cudaStream_t st, bool *dense);
 int  ordinals_launch(const agb_desc &d, Workspace &W, const void *d_text, uint64_t n, agb_record *d_records, uint64_t capacity, cudaStream_t st, bool blocks_counted = false);
 int  ordinals_reserve(const agb_desc &d, Workspace &W, uint64_t n);
+/* the ordinals of a set: delimiter ends per file into set_stats, every record's j counted from its own file's start */
+int  ordinals_set_launch(const agb_desc &d, Workspace &W, const void *d_text, const SetFile *d_files, const SetTile *d_ord_tiles,
+                         uint64_t ord_tiles, unsigned long long *d_stats, agb_record *d_records, uint64_t capacity, cudaStream_t st);
+/* a block of a SET kernel: its tile's file, and the text bounds of that file */
+__device__ __forceinline__ void set_enter(const SetFile *files, const SetTile *tiles, const uint8_t *&text, uint64_t &n,
+                                          uint64_t &tile, uint32_t &file)
+{
+	const SetTile t = tiles[blockIdx.x];
+	const SetFile f = files[t.file];
+	text += f.off; n = f.n; tile = t.tile; file = t.file;
+}
 #endif

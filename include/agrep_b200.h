@@ -136,7 +136,7 @@ typedef struct agb_record {
 	int64_t end;
 	int64_t ordinal;
 	int32_t level;
-	int32_t pad;
+	int32_t pad;              /* agb_scan_set: the index of the record's file; 0 from every other scan */
 } agb_record;
 
 enum { AGB_WANT_COUNT = 0, AGB_WANT_RECORDS = 1, AGB_WANT_ORDINALS = 2, AGB_WANT_LEVELS = 4 };
@@ -199,6 +199,20 @@ int  agb_scan_host_windowed(const agb_pattern *p, const void *h_text, uint64_t n
                             agb_record *records, uint64_t capacity, agb_result *res);
 int  agb_scan_fd_windowed(const agb_pattern *p, int fd, uint64_t window_bytes, int want,
                           agb_record *records, uint64_t capacity, agb_result *res);
+
+/* ---- a set of files in one device pass (`agrep pattern *.c`) ----
+ * File i is the text h_texts[i][0..sizes[i]) (host memory; NULL only with size 0), framed as a whole text is: the virtual
+ * '\n' in front of it, its delimiter appended behind it, j's start-with-delimiter rule, the phantom record at its end
+ * dropped.  per_file[i] (n_files entries) holds what agb_scan_host on file i alone returns -- n_matched, level_hist,
+ * n_closes -- with n_records / truncated as for a list of the room left behind the files before it; n_flagged and the
+ * times are 0.  total: the sums, n_records / truncated of the whole list.
+ * records: ONE ordered list, file 0's records, then file 1's, ...; cut after the first `capacity` records of the set.
+ * Each record's begin, end and ordinal are relative to its own file, and its `pad` field holds the file's index.
+ * The files go to the device together (each at a 16-byte boundary) and are scanned by one sequence of launches whatever
+ * their number.  A set that does not fit in device memory (or in AGB_MAX_TEXT_BYTES) is refused with AGB_ERR_NOMEM:
+ * batching is the caller's job.  n_files == 0 is valid only with NULL arrays. */
+int  agb_scan_set(const agb_pattern *p, const void *const *h_texts, const uint64_t *sizes, uint32_t n_files, int want,
+                  agb_record *records, uint64_t capacity, agb_result *per_file, agb_result *total);
 
 /* ---- a text kept in HBM across scans ----
  * exec() scans the same file up to K + 2 times under -B (agrep.c:3582-3728); the drop-in layer uploads it once.
