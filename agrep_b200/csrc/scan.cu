@@ -180,7 +180,8 @@ static int list_stage(const agb_desc &d, Workspace &W, RecParams &P, bool want_l
  * the dense form walks the bitmap, one thread per word.
  * refined: stage 1.5 ran -- the survivors are in W.bitmap2, their per-range counts in W.range_counts, and nothing
  * here needs the host to know how many there are (the list is sized by W.cand_hint / a fraction of the chunks; the
- * caller checks totals[12] against W.cand_cap afterwards and comes back with refined_retry set if it was too small). */
+ * caller, stages_after_front, reads totals[12] back and, if it exceeds W.cand_cap, calls this again -- with the list
+ * sized from that count, or with use_front off for the every-byte form when the survivors are dense). */
 static int records_launch(const agb_desc &d, Workspace &W, const void *d_text, uint64_t n, bool use_front, bool refined, int want,
                           int want_level, agb_record *d_records, uint64_t capacity, cudaStream_t st, const ShardInfo *sh)
 {
@@ -499,7 +500,9 @@ static int adaptive_plan(const agb_desc &d, Workspace &W, const void *d_text, ui
 /* everything after stage 1, on one stream: stage 1.5, the record stage, the ordinals, the result read-back (the one
  * host synchronisation of a scan).  The candidate list of the list form is sized without asking the device how many
  * survivors there are; should it turn out too small (totals[12] > capacity, seen in the read-back) the record stage
- * alone is run again with the right size -- or in its every-byte form when the survivors are dense. */
+ * and the ordinals are run again, the list with the right size -- or in its every-byte form when the survivors are
+ * dense.  Stage 1's outputs (the bitmap, the delimiter counts per block) are reused as they are, so no pass after
+ * stage 1 may change them. */
 /* shard.cu: the delimiter counts of the halos and the run check of the left halo, into totals[16..18] (read back with the rest) */
 int shard_aux_enqueue(const agb_desc &d, Workspace &W, const uint8_t *text, uint64_t n, const ShardInfo *sh, bool ordinals, cudaStream_t st);
 
