@@ -12,6 +12,8 @@ PLAN_ALL, PLAN_ANCHORS = 0, 1
 ENGINE_NAMES = {0: "bitap", 1: "asearch", 2: "asearch0", 3: "asearch1", 4: "sgrep_bm", 5: "regex"}
 ENGINE_REGEX = 5
 REGEX_MAXPOS = 63
+WIDE_WORDS = 5
+WIDE_MAXPOS = 64 * WIDE_WORDS - 1
 
 
 class Options(C.Structure):
@@ -36,11 +38,17 @@ class Desc(C.Structure):
                 ("anchor", C.c_uint32 * AGB_MAXANCHOR), ("anchor_fold", C.c_uint32), ("anchor_mask", C.c_uint32),
                 ("refine", C.c_int32), ("pat_len", C.c_int32), ("anchor_off", C.c_int32 * AGB_MAXANCHOR),
                 ("n_anchors3", C.c_int32), ("anchor3", C.c_uint32 * 4), ("anchor3_off", C.c_int32 * 4), ("adaptive", C.c_int32),
-                ("delim_fold", C.c_uint8 * (2 * AGB_MAXDELIM + 2)), ("pair_plan", C.c_uint8), ("pad_", C.c_uint8)]
+                ("delim_fold", C.c_uint8 * (2 * AGB_MAXDELIM + 2)), ("pair_plan", C.c_uint8), ("wide", C.c_uint8)]
 
 
 class Regex(C.Structure):
     _fields_ = [("follow", C.c_uint64 * (REGEX_MAXPOS + 1)), ("head", C.c_int32), ("tail", C.c_int32), ("pad", C.c_int32 * 2)]
+
+
+class Wide(C.Structure):
+    _W = C.c_uint64 * WIDE_WORDS
+    _fields_ = [("mask", _W * 256), ("init0", _W), ("init1", _W), ("noerr", _W), ("endpos", _W),
+                ("dendpos", _W), ("dmask", _W), ("reset", _W), ("start", _W)]
 
 
 class Record(C.Structure):
@@ -60,7 +68,7 @@ class CorpusSpec(C.Structure):
 
 
 EXPORTS = ["agb_fill_ordinals", "agb_compile", "agb_pattern_free", "agb_pattern_desc", "agb_pattern_from_desc", "agb_scan_device",
-           "agb_pattern_regex", "agb_pattern_from_regex",
+           "agb_pattern_regex", "agb_pattern_from_regex", "agb_pattern_wide",
            "agb_scan_host", "agb_scan_fd", "agb_scan_host_windowed", "agb_scan_fd_windowed", "agb_scan_set", "agb_bestmatch_device", "agb_corpus_fill_device", "agb_corpus_fill_host",
            "agb_last_error", "agb_device_count", "agb_set_device", "agb_version", "agb_kernel_launches", "agb_shutdown",
            "agb_text_from_host", "agb_text_from_fd", "agb_text_free", "agb_text_size", "agb_text_device", "agb_scan_text",
@@ -95,6 +103,8 @@ def lib():
     L.agb_pattern_from_desc.argtypes = [C.POINTER(Desc), C.POINTER(C.c_void_p), C.c_char_p, C.c_size_t]
     L.agb_pattern_regex.argtypes = [C.c_void_p]
     L.agb_pattern_regex.restype = C.POINTER(Regex)
+    L.agb_pattern_wide.argtypes = [C.c_void_p]
+    L.agb_pattern_wide.restype = C.POINTER(Wide)
     L.agb_pattern_from_regex.argtypes = [C.POINTER(Desc), C.POINTER(Regex), C.POINTER(C.c_void_p), C.c_char_p, C.c_size_t]
     L.agb_scan_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(Result)]
     L.agb_scan_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_uint64, C.POINTER(Result)]

@@ -8,7 +8,7 @@ import ctypes as C
 import os
 import stat
 from . import _lib
-from ._lib import (Options, Desc, Regex, Record, Result, CorpusSpec, WANT_COUNT, WANT_RECORDS, WANT_ORDINALS, WANT_LEVELS,
+from ._lib import (Options, Desc, Regex, Wide, Record, Result, CorpusSpec, WANT_COUNT, WANT_RECORDS, WANT_ORDINALS, WANT_LEVELS,
                    PLAN_ALL, PLAN_ANCHORS, ENGINE_NAMES, ENGINE_REGEX)
 
 
@@ -53,6 +53,13 @@ class Pattern:
         """the follow sets of a regular expression (a copy), None for every other engine"""
         r = _lib.lib().agb_pattern_regex(self._h)
         return Regex.from_buffer_copy(r.contents) if r else None
+
+    @property
+    def wide(self):
+        """the 320-bit words of a simple literal of more than 63 positions (a copy; word 0 = bits 0..63 of each row),
+        None for every other pattern"""
+        w = _lib.lib().agb_pattern_wide(self._h)
+        return Wide.from_buffer_copy(w.contents) if w else None
 
     def __del__(self):
         try:

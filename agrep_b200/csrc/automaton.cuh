@@ -2,6 +2,7 @@
 #ifndef AGB_AUTOMATON_CUH
 #define AGB_AUTOMATON_CUH
 #include "scan_internal.cuh"
+#include <type_traits>
 
 /* ================================================================================================
  * shared device pieces of stages 1.5 and 2: the recurrence, the match test, the text reader
@@ -22,6 +23,32 @@ template <> __device__ __forceinline__ uint32_t shift1<uint32_t>(uint32_t x)
 	return r;
 }
 
+/* a 320-bit row (agb_wide: a simple literal of more than 63 positions, k = 0), word 0 = bits 0..63.  The kernels only
+ * AND/OR/complement/compare rows and shift them right by one, so this is all a row needs. */
+struct Wide {
+	uint64_t w[AGB_WIDE_WORDS];
+	Wide() = default;
+	__device__ __forceinline__ Wide(int z) { w[0] = (uint64_t)(uint32_t)z; _Pragma("unroll") for (int i = 1; i < AGB_WIDE_WORDS; i++) w[i] = 0; }
+	__device__ __forceinline__ static Wide load(const uint64_t (&x)[AGB_WIDE_WORDS]) { Wide r; _Pragma("unroll") for (int i = 0; i < AGB_WIDE_WORDS; i++) r.w[i] = x[i]; return r; }
+	__device__ __forceinline__ explicit operator bool() const { uint64_t o = 0; _Pragma("unroll") for (int i = 0; i < AGB_WIDE_WORDS; i++) o |= w[i]; return o != 0; }
+#define WIDE_OP(op) \
+	__device__ __forceinline__ friend Wide operator op(const Wide &a, const Wide &b) { Wide r; _Pragma("unroll") for (int i = 0; i < AGB_WIDE_WORDS; i++) r.w[i] = a.w[i] op b.w[i]; return r; } \
+	__device__ __forceinline__ Wide &operator op##=(const Wide &b) { _Pragma("unroll") for (int i = 0; i < AGB_WIDE_WORDS; i++) w[i] op##= b.w[i]; return *this; }
+	WIDE_OP(&) WIDE_OP(|)
+#undef WIDE_OP
+	__device__ __forceinline__ Wide operator~() const { Wide r; _Pragma("unroll") for (int i = 0; i < AGB_WIDE_WORDS; i++) r.w[i] = ~w[i]; return r; }
+	__device__ __forceinline__ friend bool operator==(const Wide &a, const Wide &b) { uint64_t o = 0; _Pragma("unroll") for (int i = 0; i < AGB_WIDE_WORDS; i++) o |= a.w[i] ^ b.w[i]; return o == 0; }
+	__device__ __forceinline__ friend bool operator!=(const Wide &a, const Wide &b) { return !(a == b); }
+};
+template <> __device__ __forceinline__ Wide shift1<Wide>(Wide x)
+{
+	Wide r;
+#pragma unroll
+	for (int i = 0; i < AGB_WIDE_WORDS - 1; i++) r.w[i] = (x.w[i] >> 1) | (x.w[i + 1] << 63);
+	r.w[AGB_WIDE_WORDS - 1] = x.w[AGB_WIDE_WORDS - 1] >> 1;
+	return r;
+}
+
 template <typename T> struct DevConsts {
 	T init1, noerr, endpos, dendpos;
 	int L, k, and_mode, inverse, kind, ci, cs, cd;
@@ -36,15 +63,24 @@ template <typename T, int NR> struct RecShared {
 	int start_closes;
 };
 
+/* wide: the words come from the agb_wide table in device memory (RecParams.rx_tab), the rest from the descriptor */
 template <typename T, int NR>
-__device__ __forceinline__ void shared_init(RecShared<T, NR> &S, DevConsts<T> &C, const agb_desc *D, int nthreads)
+__device__ __forceinline__ void shared_init(RecShared<T, NR> &S, DevConsts<T> &C, const agb_desc *D, int nthreads, const void *wide = nullptr)
 {
-	for (int i = threadIdx.x; i < 256; i += nthreads) S.mask[i] = mirror<T>((T)D->mask[i]);
+	if constexpr (std::is_same<T, Wide>::value) {
+		static_assert(NR == 1, "320-bit rows are k = 0 only");
+		const agb_wide *X = static_cast<const agb_wide *>(wide);
+		for (int i = threadIdx.x; i < 256; i += nthreads) S.mask[i] = Wide::load(X->mask[i]);
+		if (threadIdx.x == 0) { S.reset[0] = Wide::load(X->reset); S.start[0] = Wide::load(X->start); }
+		C.init1 = Wide::load(X->init1); C.noerr = Wide::load(X->noerr); C.endpos = Wide::load(X->endpos); C.dendpos = Wide::load(X->dendpos);
+	} else {
+		for (int i = threadIdx.x; i < 256; i += nthreads) S.mask[i] = mirror<T>((T)D->mask[i]);
+		if (threadIdx.x < NR) { S.reset[threadIdx.x] = mirror<T>((T)D->reset[threadIdx.x]); S.start[threadIdx.x] = mirror<T>((T)D->start[threadIdx.x]); }
+		C.init1 = mirror<T>((T)D->init1); C.noerr = mirror<T>((T)D->noerr); C.endpos = mirror<T>((T)D->endpos); C.dendpos = mirror<T>((T)D->dendpos);
+	}
 	if (threadIdx.x == 0) { S.mask[256] = 0; S.start_closes = D->start_closes; }
-	if (threadIdx.x < NR) { S.reset[threadIdx.x] = mirror<T>((T)D->reset[threadIdx.x]); S.start[threadIdx.x] = mirror<T>((T)D->start[threadIdx.x]); }
 	if (threadIdx.x < 2 * AGB_MAXDELIM + 2) { S.dfold[threadIdx.x] = D->delim_fold[threadIdx.x]; S.delim[threadIdx.x] = D->delim[threadIdx.x] | D->delim_fold[threadIdx.x]; }
 	if (threadIdx.x <= AGB_MAXERR) S.hist[threadIdx.x] = 0;
-	C.init1 = mirror<T>((T)D->init1); C.noerr = mirror<T>((T)D->noerr); C.endpos = mirror<T>((T)D->endpos); C.dendpos = mirror<T>((T)D->dendpos);
 	C.L = D->L; C.k = D->k; C.and_mode = D->and_mode; C.inverse = D->inverse; C.kind = D->delim_kind;
 	C.ci = D->cost_i; C.cs = D->cost_s; C.cd = D->cost_d;
 	__syncthreads();

@@ -477,7 +477,7 @@ __global__ void __launch_bounds__(EXR_THREADS) k_exact_reduce(const uint32_t *su
 
 bool exact_count_usable(const agb_desc &d)
 {
-	if (!front_usable(d) || d.k != 0 || d.n_anchors != 1 || d.n_anchors3 || d.pat_len != d.anchor_len || d.inverse || d.L != 1 || d.and_mode) return false;
+	if (!front_usable(d) || d.wide || d.k != 0 || d.n_anchors != 1 || d.n_anchors3 || d.pat_len != d.anchor_len || d.inverse || d.L != 1 || d.and_mode) return false;
 	if (d.engine != AGB_ENGINE_BITAP && d.engine != AGB_ENGINE_SGREP_BM) return false;
 	if (d.wildmask || d.init1 == ~0ull || d.delim_fold[0]) return false;
 	for (int t = 0; t < d.anchor_len; t++) {

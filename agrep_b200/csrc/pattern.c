@@ -5,7 +5,8 @@
  * (preproce.c:137-341: delimiter + separator + -w/-x wrap + meta characters) and maskgen()
  * (maskgen.c:26-269: Mask[], Init[0], Init1, NO_ERR_MASK, endposition, D_endpos, wildmask) -- but is
  * organised as one pass over the user's pattern that emits automaton positions with 256-bit classes,
- * in 64-bit words (the reference stops at 32 positions, maskgen.c:201-208).
+ * in 64-bit words (the reference stops at 32 positions, maskgen.c:201-208), or in the 320-bit words of agb_wide for a
+ * simple literal of more than 63 positions at k = 0 (sgrep()'s bm()/monkey(), which take up to 255 characters).
  *
  * It also derives what only the device path needs: the constant post-delimiter rows (asearch.c:175-186),
  * the delimiter kind, and the pigeonhole anchor plan for the front-end kernel.
@@ -34,8 +35,9 @@ typedef struct {
 } pos_t;
 
 typedef struct {
-	pos_t p[WIDTH + 4];
+	pos_t p[AGB_WIDE_MAXPOS + 4];
 	int n;               /* positions so far (1-based: p[1..n]) */
+	int wide_ok;         /* up to AGB_WIDE_MAXPOS positions (a simple literal at k = 0), else up to WIDTH - 1 */
 	int no_error, even;
 	int or_seen, and_mode, nparts;
 } build_t;
@@ -55,7 +57,7 @@ static int is_alnum(int c) { return is_alpha(c) || (c >= '0' && c <= '9'); }
 static pos_t *new_pos(build_t *b)
 {
 	pos_t *p;
-	if (b->n + 1 > WIDTH - 1) return NULL;     /* M <= W-1: one always-on feed bit above the field */
+	if (b->n + 1 > (b->wide_ok ? AGB_WIDE_MAXPOS : WIDTH - 1)) return NULL;     /* M <= W-1: one always-on feed bit above the field */
 	p = &b->p[++b->n];
 	memset(p, 0, sizeof *p);
 	p->lit = -1;
@@ -255,6 +257,43 @@ static int has_border(const unsigned char *d, int L)
 /* the delimiter as the device compares it: letters that accept both cases in lower case */
 static void folded_delim(const agb_desc *d, unsigned char *out) { int p; for (p = 0; p < d->L; p++) out[p] = (unsigned char)(d->delim[p] | d->delim_fold[p]); }
 
+static int derive(agb_desc *d, agb_wide *w, char *err, size_t errlen);
+
+/* a row of agb_wide: bit i in word i / 64 */
+static void w_set(uint64_t *w, int bit) { w[bit >> 6] |= 1ull << (bit & 63); }
+static int  w_has(const uint64_t *w, int bit) { return (int)(w[bit >> 6] >> (bit & 63) & 1); }
+static void w_shr1(const uint64_t *x, uint64_t *r)
+{
+	int i;
+	for (i = 0; i < AGB_WIDE_WORDS; i++) r[i] = (x[i] >> 1) | (i + 1 < AGB_WIDE_WORDS ? x[i + 1] << 63 : 0);
+}
+
+/* the words of finish() below in 320-bit rows, for a simple literal (SGREP_BM: no '#', no -p, no LUT, one separator).
+ * The "everywhere but" masks fill the words up to the one that holds the feed bit M, so that M <= 63 gives the 64-bit
+ * words in word 0 and zeros above */
+static int finish_wide(const build_t *b, agb_desc *d, agb_wide *w, char *err, size_t errlen)
+{
+	const int M = b->n, L = d->L, top = M / 64 + 1;
+	int p, c, i;
+	memset(w, 0, sizeof *w);
+	for (i = 0; i < top; i++) { w->noerr[i] = ~0ull; w->dmask[i] = ~0ull; }
+	for (i = M; i < 64 * top; i++) w_set(w->init0, i);
+	w_set(w->endpos, 0);                                                       /* endp = (sep << 1) + 1 */
+	for (p = 1; p <= M; p++) {
+		const pos_t *q = &b->p[p];
+		if (q->is_sep) { w_set(w->init0, M - p); w_set(w->endpos, M - p + 1); }
+		if (q->prot) w->noerr[(M - p) >> 6] &= ~(1ull << ((M - p) & 63));
+		for (c = 0; c < 256; c++) if (cls_has(q, c)) w_set(w->mask[c], M - p);
+	}
+	for (i = 0; i < AGB_WIDE_WORDS; i++) w->init1[i] = w->init0[i] | w->endpos[i];
+	if (w_has(w->endpos, M - L)) { w_set(w->dendpos, M - L); w->endpos[(M - L) >> 6] ^= 1ull << ((M - L) & 63); }
+	for (p = 1; p <= L; p++) w->dmask[(M - p) >> 6] &= ~(1ull << ((M - p) & 63));
+	d->M = M;
+	d->and_mode = b->and_mode;
+	d->wide = 1;                                                               /* (the 64-bit words stay zero) */
+	return derive(d, w, err, errlen);
+}
+
 /* derive the words from the positions (maskgen.c:218-257 with WORD = 64, LSB aligned) and the device-only constants */
 static int finish(build_t *b, agb_desc *d, const agb_options *o, const unsigned char *lut, char *err, size_t errlen)
 {
@@ -281,7 +320,7 @@ static int finish(build_t *b, agb_desc *d, const agb_options *o, const unsigned 
 	d->dmask = ~d->dmask;
 	d->and_mode = b->and_mode;
 	if (o->ins_free) d->init1 = ~0ull;                                         /* bitap.c:123, asearch.c:49 */
-	return agbi_derive(d, err, errlen);
+	return derive(d, NULL, err, errlen);
 }
 
 /* post-delimiter rows: asearch.c:175-186 / bitap.c:223-225 / asearch1.c:150-158.  Row 0 is masked with
@@ -303,14 +342,22 @@ static void reset_rows(const agb_desc *d, uint64_t cm, uint64_t *A)
 	}
 }
 
-/* everything the device path needs beyond the reference's words */
-int agbi_derive(agb_desc *d, char *err, size_t errlen)
+/* does position p of the delimiter accept byte c? */
+static int delim_accepts(const agb_desc *d, const agb_wide *w, int c, int p)
+{
+	return w ? w_has(w->mask[c], d->M - p) : (int)(d->mask[c] >> (d->M - p) & 1);
+}
+
+/* everything the device path needs beyond the reference's words; w: the words are those of agb_wide (k = 0) */
+int agbi_derive(agb_desc *d, char *err, size_t errlen) { return derive(d, NULL, err, errlen); }
+
+static int derive(agb_desc *d, agb_wide *w, char *err, size_t errlen)
 {
 	int L = d->L, p, r;
 	uint64_t B[2 * AGB_MAXERR + 1], A[2 * AGB_MAXERR + 1];
-	if (L < 1 || L > AGB_MAXDELIM || d->M < L + 1 || d->M > WIDTH - 1) FAIL("bad descriptor (M=%d, L=%d)", d->M, L);
-	if (d->k < 0 || d->k > AGB_MAXERR) FAIL("bad descriptor (k=%d)", d->k);
-	if (!d->dendpos) FAIL("internal: delimiter end bit missing");
+	if (L < 1 || L > AGB_MAXDELIM || d->M < L + 1 || d->M > (w ? AGB_WIDE_MAXPOS : WIDTH - 1)) FAIL("bad descriptor (M=%d, L=%d)", d->M, L);
+	if (d->k < 0 || d->k > AGB_MAXERR || (w && d->k)) FAIL("bad descriptor (k=%d)", d->k);
+	if (w ? !w_has(w->dendpos, d->M - L) : !d->dendpos) FAIL("internal: delimiter end bit missing");
 	/* the device also recognises delimiters away from the automaton (record starts, ordinals), by their bytes: position p
 	 * of the delimiter must accept delim[p-1] and nothing else (-i with letters in the delimiter makes it accept both cases) */
 	/* -p (Init1 all ones, bitap.c:123) makes every position sticky, the delimiter's too: with a delimiter of two or more
@@ -319,11 +366,11 @@ int agbi_derive(agb_desc *d, char *err, size_t errlen)
 		FAIL("-p with a delimiter of more than one byte is not supported (insertions inside the delimiter would be free too)");
 	memset(d->delim_fold, 0, sizeof d->delim_fold);
 	for (p = 1; p <= L; p++) {
-		const uint64_t bit = 1ull << (d->M - p); int c, cnt = 0, lo = d->delim[p - 1] | 0x20;
-		for (c = 0; c < 256; c++) if (d->mask[c] & bit) cnt++;
-		if (cnt == 1 && (d->mask[d->delim[p - 1]] & bit)) continue;
+		int c, cnt = 0, lo = d->delim[p - 1] | 0x20;
+		for (c = 0; c < 256; c++) if (delim_accepts(d, w, c, p)) cnt++;
+		if (cnt == 1 && delim_accepts(d, w, d->delim[p - 1], p)) continue;
 		/* -i with a letter in the delimiter: both cases end the record (maskgen.c:52-58, 259-266) */
-		if (cnt == 2 && lo >= 'a' && lo <= 'z' && (d->mask[lo] & bit) && (d->mask[lo - 32] & bit)) { d->delim_fold[p - 1] = 0x20; continue; }
+		if (cnt == 2 && lo >= 'a' && lo <= 'z' && delim_accepts(d, w, lo, p) && delim_accepts(d, w, lo - 32, p)) { d->delim_fold[p - 1] = 0x20; continue; }
 		FAIL("the delimiter matches more than its own bytes here: not supported by the device record search");
 	}
 	/* delimiter recognition away from the automaton (record-start search on the device) */
@@ -334,13 +381,23 @@ int agbi_derive(agb_desc *d, char *err, size_t errlen)
 		for (p = 1; p < L; p++) if (fd[p] != fd[0]) break;
 		d->delim_kind = p < L ? 2 : 1;          /* a run such as $$, or any other self-overlap ("aba"): automaton.cuh delim_ends_at */
 	}
+	d->nrows = d->k + 1;
+	if (w) {
+		/* one row: reset_rows() and the virtual '\n' below, in 320 bits */
+		uint64_t s[AGB_WIDE_WORDS], a[AGB_WIDE_WORDS]; int i, hit = 0;
+		w_shr1(w->init0, s);
+		for (i = 0; i < AGB_WIDE_WORDS; i++) w->reset[i] = ((s[i] & w->mask[d->delim[L - 1]][i]) | (w->init1[i] & w->init0[i])) & w->dmask[i];
+		for (i = 0; i < AGB_WIDE_WORDS; i++) { a[i] = (s[i] & w->mask['\n'][i]) | (w->init1[i] & w->init0[i]); hit |= (a[i] & w->dendpos[i]) != 0; }
+		d->start_closes = hit;
+		memcpy(w->start, hit ? w->reset : a, sizeof a);
+		return 0;
+	}
 	reset_rows(d, d->mask[d->delim[L - 1]], d->reset);
 	/* the virtual '\n' in front of the text (bitap.c:140,148-149) */
 	for (r = 0; r <= d->k; r++) B[r] = d->init0;
 	agbi_step(d, B, A, d->mask['\n']);
 	if (A[0] & d->dendpos) { d->start_closes = 1; memcpy(d->start, d->reset, sizeof(uint64_t) * (size_t)(d->k + 1)); }
 	else { d->start_closes = 0; memcpy(d->start, A, sizeof(uint64_t) * (size_t)(d->k + 1)); }
-	d->nrows = d->k + 1;
 	return 0;
 }
 
@@ -457,7 +514,8 @@ static void plan_anchors(const build_t *b, agb_desc *d, const agb_options *o, in
 			if (dup) continue;
 			d->anchor[d->n_anchors] = val; d->anchor_off[d->n_anchors++] = pos[p] - (d->L + 2);
 		}
-		d->refine = (b->nparts == 1 && !b->and_mode && !b->or_seen && d->wildmask == 0) ? 1 : 0;
+		/* (320-bit rows: no stage 1.5 -- the record stage judges the flagged chunks) */
+		d->refine = (b->nparts == 1 && !b->and_mode && !b->or_seen && d->wildmask == 0 && !d->wide) ? 1 : 0;
 		/* the planner in scan.cu re-derives plans from the literal positions alone: not for a plan that leans on classes */
 		if (classes) d->adaptive = 0;
 		if (d->inverse) d->plan = AGB_PLAN_ALL;       /* (the anchors stay in the descriptor for the complement count) */
@@ -729,10 +787,10 @@ static int rx_build(const unsigned char *s, int m, const agb_options *o, agb_des
 
 int agbi_build(const char *pattern, const agb_options *o, agb_desc *d, char *err, size_t errlen)
 {
-	return agbi_build_rx(pattern, o, d, NULL, err, errlen);
+	return agbi_build_rx(pattern, o, d, NULL, NULL, err, errlen);
 }
 
-int agbi_build_rx(const char *pattern, const agb_options *o, agb_desc *d, agb_regex *rx, char *err, size_t errlen)
+int agbi_build_rx(const char *pattern, const agb_options *o, agb_desc *d, agb_regex *rx, agb_wide *wide, char *err, size_t errlen)
 {
 	build_t *b; int m, rc, notsgrep = 0, simple, jump, sg; unsigned char lut[256];
 	const unsigned char *s = (const unsigned char *)pattern;
@@ -777,6 +835,7 @@ int agbi_build_rx(const char *pattern, const agb_options *o, agb_desc *d, agb_re
 		/* sgrep.c:289-320 + bm() :741-755: literal compared under TR[] (ASCII case folded, unconditional,
 		 * sgrep.c:226-236); -w = neither neighbour isalnum().  Stated as an exact automaton. */
 		int i;
+		b->wide_ok = wide != NULL;
 		if (o->wordbound) { pos_t *p = new_pos(b); int c; if (p) { p->prot = 1; for (c = 0; c < 256; c++) if (!is_alnum(c)) cls_set(p, c); } else rc = AGB_ERR_PATTERN; }
 		for (i = 0; i < m && !rc; i++) {
 			int c = s[i]; pos_t *p;
@@ -799,6 +858,8 @@ int agbi_build_rx(const char *pattern, const agb_options *o, agb_desc *d, agb_re
 	}
 	if (rc) { if (err && errlen && !err[0]) snprintf(err, errlen, "pattern too long (has > %d chars)", WIDTH); free(b); return AGB_ERR_PATTERN; }
 	if (d->engine == AGB_ENGINE_BITAP && o->nocase) { agbi_lut_lower1(lut); rc = finish(b, d, o, lut, err, errlen); }
+	else if (b->wide_ok && (b->n > WIDTH - 1 || (getenv("AGB_FORCE_WIDE") && atoi(getenv("AGB_FORCE_WIDE")) == 1)))
+		rc = finish_wide(b, d, wide, err, errlen);                             /* (AGB_FORCE_WIDE=1: every simple literal, for tests) */
 	else rc = finish(b, d, o, NULL, err, errlen);
 	if (!rc) plan_anchors(b, d, o, d->engine == AGB_ENGINE_SGREP_BM);
 	free(b);
@@ -813,13 +874,14 @@ int agb_compile(const char *pattern, const agb_options *opt, agb_pattern **out, 
 	if (!out) return AGB_ERR_ARG;
 	p = (agb_pattern *)calloc(1, sizeof *p);
 	if (!p) return AGB_ERR_NOMEM;
-	rc = agbi_build_rx(pattern, opt, &p->d, &p->rx, err, errlen);
+	rc = agbi_build_rx(pattern, opt, &p->d, &p->rx, &p->wide, err, errlen);
 	if (rc) { free(p); *out = NULL; return rc; }
 	*out = p;
 	return AGB_OK;
 }
 
 const agb_regex *agb_pattern_regex(const agb_pattern *p) { return (p && p->d.engine == AGB_ENGINE_REGEX) ? &p->rx : NULL; }
+const agb_wide *agb_pattern_wide(const agb_pattern *p) { return (p && p->d.wide) ? &p->wide : NULL; }
 
 int agb_pattern_from_regex(const agb_desc *d, const agb_regex *rx, agb_pattern **out, char *err, size_t errlen)
 {
@@ -829,6 +891,7 @@ int agb_pattern_from_regex(const agb_desc *d, const agb_regex *rx, agb_pattern *
 	p = (agb_pattern *)calloc(1, sizeof *p);
 	if (!p) return AGB_ERR_NOMEM;
 	p->d = *d; p->rx = *rx;
+	p->d.wide = 0;
 	/* nothing outside positions 0..M */
 	if (p->d.M >= 1 && p->d.M <= AGB_REGEX_MAXPOS) {
 		const uint64_t field = (p->d.M == 63) ? ~0ull : (2ull << p->d.M) - 1;
@@ -854,6 +917,7 @@ int agb_pattern_from_desc(const agb_desc *d, agb_pattern **out, char *err, size_
 	}
 	if (p->d.n_anchors3 < 0 || p->d.n_anchors3 > 2 || p->d.plan != AGB_PLAN_ANCHORS) p->d.n_anchors3 = 0;
 	p->d.pair_plan = 0;
+	p->d.wide = 0;                 /* (the words must be in the descriptor: a descriptor of 320-bit rows is refused below) */
 	rc = agbi_derive(&p->d, err, errlen);
 	if (rc) { free(p); *out = NULL; return rc; }
 	*out = p;

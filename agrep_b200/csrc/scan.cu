@@ -136,20 +136,30 @@ static int ws_upload_desc(Workspace &W, const agb_desc &d, cudaStream_t st)
 	return AGB_OK;
 }
 
-/* AGB_ENGINE_REGEX: the pattern's Next tables to the device (regex.cu reads them from RecParams.rx_tab) */
-static int regex_prepare(Workspace &W, const agb_desc &d, const agb_regex *rx, cudaStream_t st)
+/* what the descriptor cannot hold, to the device, where the record stage reads it from RecParams.rx_tab: the Next tables
+ * of AGB_ENGINE_REGEX (regex.cu), or the words of 320-bit rows (agb_desc.wide, records_wide.cu).  px: the pattern that
+ * holds them (NULL: a descriptor that needs neither) */
+static_assert(sizeof(agb_wide) <= sizeof(Workspace::h_regex), "the wide words travel in the regex table buffer");
+static int tables_prepare(Workspace &W, const agb_desc &d, const agb_pattern *px, cudaStream_t st)
 {
-	if (d.engine != AGB_ENGINE_REGEX) return AGB_OK;
-	if (!rx) { snprintf(g_err, sizeof g_err, "a regular expression needs its follow sets (agb_pattern_from_regex)"); return AGB_ERR_ARG; }
+	if (d.engine != AGB_ENGINE_REGEX && !d.wide) return AGB_OK;
+	const agb_regex *rx = agb_pattern_regex(px);
+	const agb_wide *wide = agb_pattern_wide(px);
+	if (d.wide ? !wide : !rx) {
+		snprintf(g_err, sizeof g_err, d.wide ? "a literal of 320-bit rows needs its words (agb_compile)" : "a regular expression needs its follow sets (agb_pattern_from_regex)");
+		return AGB_ERR_ARG;
+	}
 	if (!W.d_regex) CUDA_TRY(cudaMalloc(&W.d_regex, sizeof W.h_regex));
 	uint64_t tab[8 * 256];
-	const size_t bytes = regex_tables(d, *rx, tab);
+	size_t bytes;
+	if (d.wide) { memcpy(tab, wide, sizeof *wide); bytes = sizeof *wide; }
+	else bytes = regex_tables(d, *rx, tab);
 	if (bytes != W.regex_bytes || memcmp(tab, W.h_regex, bytes) != 0) {
 		CUDA_TRY(cudaMemcpyAsync(W.d_regex, tab, bytes, cudaMemcpyHostToDevice, st));
 		CUDA_TRY(cudaStreamSynchronize(st));     /* tab is on this stack */
 		memcpy(W.h_regex, tab, bytes); W.regex_bytes = bytes;
 	}
-	W.regex_tail = rx->tail;
+	if (rx) W.regex_tail = rx->tail;
 	return AGB_OK;
 }
 
@@ -543,7 +553,7 @@ static bool complement_usable(const agb_desc &d)
 
 int scan_device_impl(const agb_desc &d_in, const void *d_text, uint64_t n, int want, int want_level,
                      agb_record *d_records, uint64_t capacity, cudaStream_t st, agb_result *res, const ShardInfo *sh,
-                     const agb_regex *rx)
+                     const agb_pattern *px)
 {
 	if (!res) return AGB_ERR_ARG;
 	memset(res, 0, sizeof *res);
@@ -559,7 +569,7 @@ int scan_device_impl(const agb_desc &d_in, const void *d_text, uint64_t n, int w
 		 * agrep.c:3811 drops).  The newlines are counted by the same pass (j at EOF = newlines + appended + virtual). */
 		agb_desc pos = d_in; pos.inverse = 0; pos.plan = AGB_PLAN_ANCHORS;
 		agb_result r;
-		int rc = scan_device_impl(pos, d_text, n, AGB_WANT_COUNT | AGB_WANT_ORDINALS, -1, nullptr, 0, st, &r, nullptr); if (rc) return rc;
+		int rc = scan_device_impl(pos, d_text, n, AGB_WANT_COUNT | AGB_WANT_ORDINALS, -1, nullptr, 0, st, &r, nullptr, px); if (rc) return rc;
 		unsigned char last = 0;
 		CUDA_TRY(cudaMemcpyAsync(&last, (const uint8_t *)d_text + n - 1, 1, cudaMemcpyDeviceToHost, st));
 		CUDA_TRY(cudaStreamSynchronize(st));
@@ -589,7 +599,7 @@ int scan_device_impl(const agb_desc &d_in, const void *d_text, uint64_t n, int w
 		return AGB_OK;
 	}
 	rc = ws_upload_desc(W, d, st); if (rc) return rc;
-	rc = regex_prepare(W, d, rx, st); if (rc) return rc;
+	rc = tables_prepare(W, d, px, st); if (rc) return rc;
 	CUDA_TRY(cudaMemsetAsync(W.totals, 0, 16 * sizeof(unsigned long long), st));
 	CUDA_TRY(cudaEventRecord(W.e0, st));
 	bool use_front = front_usable(d) && n > 0;
@@ -609,7 +619,7 @@ extern "C" int agb_scan_device(const agb_pattern *p, const void *d_text, uint64_
                                agb_record *d_records, uint64_t capacity, void *stream, agb_result *res)
 {
 	if (!p) return AGB_ERR_ARG;
-	return scan_device_impl(p->d, d_text, n, want, -1, d_records, capacity, (cudaStream_t)stream, res, nullptr, agb_pattern_regex(p));
+	return scan_device_impl(p->d, d_text, n, want, -1, d_records, capacity, (cudaStream_t)stream, res, nullptr, p);
 }
 
 /* Host text -> HBM -> scan: the replacement of the fill_buf()/read(2) loop (bitap.c:143,450-477).  The text is moved in
@@ -796,7 +806,7 @@ static uint64_t max_text_bytes(void)
  * the caller scans it in windows instead */
 #define SCAN_NEEDS_WINDOWS 1
 
-static int scan_stream_impl(const agb_desc &d, const agb_regex *rx, SliceSource &src, int want,
+static int scan_stream_impl(const agb_desc &d, const agb_pattern *px, SliceSource &src, int want,
                             agb_record *records, uint64_t capacity, agb_result *res)
 {
 	memset(res, 0, sizeof *res);
@@ -820,7 +830,7 @@ static int scan_stream_impl(const agb_desc &d, const agb_regex *rx, SliceSource 
 	rc = host_ensure(H, src); if (rc) return rc;
 	CUDA_TRY(dev_reserve(&H.rec, &H.rec_cap, (want & AGB_WANT_RECORDS) ? capacity * sizeof(agb_record) : 0));
 	rc = ws_upload_desc(W, d, H.s_comp); if (rc) return rc;
-	rc = regex_prepare(W, d, rx, H.s_comp); if (rc) return rc;
+	rc = tables_prepare(W, d, px, H.s_comp); if (rc) return rc;
 	const bool use_front = front_usable(d) && n > 0;
 	const bool count_in_front = use_front && (want & AGB_WANT_ORDINALS) && d.L == 1;
 	if (count_in_front) { rc = ordinals_prepare_blocks(d, W, n, H.s_comp); if (rc) return rc; }
@@ -879,7 +889,7 @@ static WinGeom win_geom(uint64_t n, uint64_t w, uint64_t i, uint64_t hl, uint64_
 	return g;
 }
 
-static int scan_windowed(const agb_desc &d, const agb_regex *rx, SliceSource &src, uint64_t w, int want,
+static int scan_windowed(const agb_desc &d, const agb_pattern *px, SliceSource &src, uint64_t w, int want,
                          agb_record *records, uint64_t capacity, agb_result *res)
 {
 	memset(res, 0, sizeof *res);
@@ -924,7 +934,7 @@ static int scan_windowed(const agb_desc &d, const agb_regex *rx, SliceSource &sr
 		for (;;) {
 			g = win_geom(n, w, i, hl, hr);
 			const uint64_t room = want_list ? std::min<uint64_t>(capacity - copied, B.rec_cap / sizeof(agb_record)) : 0;
-			rc = shard_window_scan(d, rx, base + g.hl, g.n_local, g.hl, g.hr, g.first, g.open_end, g.reaches_end, want,
+			rc = shard_window_scan(d, px, base + g.hl, g.n_local, g.hl, g.hr, g.first, g.open_end, g.reaches_end, want,
 			                       B.rec, room, H.s_comp, &lres, &part);
 			if (rc < 0) return rc;
 			int short_halos = rc;
@@ -992,9 +1002,9 @@ static int scan_host_any(const agb_pattern *p, const void *h_text, uint64_t n, u
 	if (!p || !res || (!h_text && n)) return AGB_ERR_ARG;
 	if ((want & AGB_WANT_RECORDS) && capacity && !records) return AGB_ERR_ARG;
 	SliceSource src(h_text, n);
-	if (window_bytes) return scan_windowed(p->d, agb_pattern_regex(p), src, window_bytes, want, records, capacity, res);
-	int rc = scan_stream_impl(p->d, agb_pattern_regex(p), src, want, records, capacity, res);
-	if (rc == SCAN_NEEDS_WINDOWS) rc = scan_windowed(p->d, agb_pattern_regex(p), src, fallback_window(), want, records, capacity, res);
+	if (window_bytes) return scan_windowed(p->d, p, src, window_bytes, want, records, capacity, res);
+	int rc = scan_stream_impl(p->d, p, src, want, records, capacity, res);
+	if (rc == SCAN_NEEDS_WINDOWS) rc = scan_windowed(p->d, p, src, fallback_window(), want, records, capacity, res);
 	return rc;
 }
 
@@ -1005,9 +1015,9 @@ static int scan_fd_any(const agb_pattern *p, int fd, uint64_t window_bytes, int 
 	SliceSource src;
 	if (fd_source(fd, src)) {
 		/* regular file: the size is known, read(2) goes straight into the pinned ring, slice by slice */
-		int rc = window_bytes ? scan_windowed(p->d, agb_pattern_regex(p), src, window_bytes, want, records, capacity, res)
-		                      : scan_stream_impl(p->d, agb_pattern_regex(p), src, want, records, capacity, res);
-		if (rc == SCAN_NEEDS_WINDOWS) rc = scan_windowed(p->d, agb_pattern_regex(p), src, fallback_window(), want, records, capacity, res);
+		int rc = window_bytes ? scan_windowed(p->d, p, src, window_bytes, want, records, capacity, res)
+		                      : scan_stream_impl(p->d, p, src, want, records, capacity, res);
+		if (rc == SCAN_NEEDS_WINDOWS) rc = scan_windowed(p->d, p, src, fallback_window(), want, records, capacity, res);
 		if (src.fd_off >= 0) lseek(fd, src.fd_off + (off_t)src.n, SEEK_SET);        /* as read(2) would have left it */
 		return rc;
 	}
@@ -1083,7 +1093,6 @@ extern "C" int agb_scan_set(const agb_pattern *p, const void *const *h_texts, co
 	for (uint32_t i = 0; i < n_files; i++)
 		if (!h_texts[i] && sizes[i]) { snprintf(g_err, sizeof g_err, "agb_scan_set: file %u has no text but %llu bytes", i, (unsigned long long)sizes[i]); return AGB_ERR_ARG; }
 	const agb_desc &d = p->d;
-	const agb_regex *rx = agb_pattern_regex(p);
 	/* the layout: file i at at[i]; its record tiles (of the kernel that runs) and its ordinals tiles (of [0, n + L)) */
 	const uint64_t rec_tile = d.engine == AGB_ENGINE_REGEX ? RX_TILE : DENSE_TILE;
 	std::vector<uint64_t> at(n_files);
@@ -1135,7 +1144,7 @@ extern "C" int agb_scan_set(const agb_pattern *p, const void *const *h_texts, co
 	CUDA_TRY(cudaMemcpyAsync(d_otiles, otiles.data(), ob, cudaMemcpyHostToDevice, H.s_comp));
 	CUDA_TRY(cudaMemsetAsync(d_stats, 0, sb, H.s_comp));
 	rc = ws_upload_desc(W, d, H.s_comp); if (rc) return rc;
-	rc = regex_prepare(W, d, rx, H.s_comp); if (rc) return rc;
+	rc = tables_prepare(W, d, p, H.s_comp); if (rc) return rc;
 	CUDA_TRY(cudaMemsetAsync(W.totals, 0, 16 * sizeof(unsigned long long), H.s_comp));
 	rc = upload(H, src, 0, bytes, H.text, need - bytes, [&](uint64_t, cudaEvent_t ev) -> int {
 		CUDA_TRY(cudaStreamWaitEvent(H.s_comp, ev, 0));
@@ -1256,7 +1265,7 @@ extern "C" int agb_scan_text(const agb_pattern *p, const agb_text *t, int want, 
 	std::lock_guard<std::mutex> lk(g_host_mu[t->dev]);
 	HostPath &H = g_host[t->dev];
 	CUDA_TRY(dev_reserve(&H.rec, &H.rec_cap, (want & AGB_WANT_RECORDS) ? capacity * sizeof(agb_record) : 0));
-	int rc = scan_device_impl(p->d, t->d, t->n, want, -1, H.rec, capacity, nullptr, res, nullptr, agb_pattern_regex(p)); if (rc) return rc;
+	int rc = scan_device_impl(p->d, t->d, t->n, want, -1, H.rec, capacity, nullptr, res, nullptr, p); if (rc) return rc;
 	if (res->n_records) CUDA_TRY(cudaMemcpy(records, H.rec, res->n_records * sizeof(agb_record), cudaMemcpyDeviceToHost));
 	return AGB_OK;
 }

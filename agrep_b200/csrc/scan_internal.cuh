@@ -2,7 +2,7 @@
  * geometry, kernel parameter blocks, the per-device workspace and the host functions that cross files.
  *   front.cu    stage 1   k_front            (anchor filter, HBM-bound)
  *   refine.cu   stage 1.5 k_refine           (local verification of anchor hits)
- *   records.cu  stage 2   k_records, k_records_dense, k_records_list
+ *   records.cu  stage 2   k_records, k_records_dense, k_records_list (records_kernel.cuh; records_wide.cu: 320-bit rows)
  *   slices.cu   stage 2   k_records_slices   (the automaton over every byte, in lockstep)
  *   regex.cu    stage 2   k_regex            (regular expressions: re()'s recurrence over every byte, tile form)
  *   aux.cu      bitmap compaction, scans, density sample, ordinals, synthetic corpus
@@ -102,7 +102,8 @@ struct RecParams {
 	 * asearch.c:175-196); unsharded: everything.  shard_last = 0: the delimiter appended behind the text (bitap.c:161-165)
 	 * is not the text's own end -- an owned record that only it closes has outrun the halo (totals[11] is raised) */
 	int64_t own_lo, own_hi; int shard_last;
-	/* regular expressions (regex.cu): the byte-sliced Next tables on the device, TAIL's epsilon move at '\n' */
+	/* regular expressions (regex.cu): the byte-sliced Next tables on the device, TAIL's epsilon move at '\n';
+	 * 320-bit rows (agb_desc.wide): the agb_wide words on the device */
 	const void *rx_tab; int rx_tail;
 	/* a set of files (agb_scan_set, the kernels' SET form): block b scans tile set_tiles[b].tile of file set_tiles[b].file */
 	const struct SetFile *set_files; const struct SetTile *set_tiles; unsigned long long *set_stats;
@@ -189,11 +190,13 @@ extern Workspace g_ws[64];
 extern std::mutex g_ws_mu[64];   /* one scan at a time per device (the workspaces are shared scratch) */
 int  scan_device_impl(const agb_desc &d, const void *d_text, uint64_t n, int want, int want_level,
                       agb_record *d_records, uint64_t capacity, cudaStream_t st, agb_result *res, const ShardInfo *sh = nullptr,
-                      const agb_regex *rx = nullptr);
+                      const agb_pattern *px = nullptr);
+/* px (here and below): the pattern that holds what its descriptor cannot -- a regular expression's follow sets, the words
+ * of 320-bit rows; NULL for a descriptor that needs neither */
 /* shard.cu: one window of the windowed scan -- the shard scan, with a halo that is too short reported as a positive code
  * (a set of HALO_SHORT_*) instead of an error; and the window's records made global on the device */
 enum { HALO_SHORT_RIGHT = 1, HALO_SHORT_LEFT = 2 };
-int  shard_window_scan(const agb_desc &d, const agb_regex *rx, const void *d_win, uint64_t n_local, uint64_t halo_left, uint64_t halo_right,
+int  shard_window_scan(const agb_desc &d, const agb_pattern *px, const void *d_win, uint64_t n_local, uint64_t halo_left, uint64_t halo_right,
                        bool first, bool open_end, bool reaches_end, int want, agb_record *d_records, uint64_t capacity,
                        cudaStream_t st, agb_result *lres, agb_shard_part *part);
 int  shard_window_rebase(agb_record *d_records, uint64_t n, long long byte_add, long long ord_add, bool ordinals, cudaStream_t st);
@@ -215,6 +218,11 @@ int  launch_dense(const agb_desc &d, const RecParams &P, unsigned grid, cudaStre
 int  launch_dense_set(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 int  launch_regex_set(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 int  launch_records_list(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
+/* records_wide.cu: the same forms for 320-bit rows (agb_desc.wide: the words in RecParams.rx_tab), which the launchers
+ * above hand over to */
+int  launch_records_wide(const RecParams &P, unsigned grid, cudaStream_t st);
+int  launch_dense_wide(const RecParams &P, unsigned grid, cudaStream_t st, bool set);
+int  launch_records_list_wide(const RecParams &P, unsigned grid, cudaStream_t st);
 int  launch_slices(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 bool slices_usable(const agb_desc &d);
 /* regex.cu: stage 2 of AGB_ENGINE_REGEX (RecParams.rx_tab set), and its tables (returns the bytes written: 32- or 64-bit words) */

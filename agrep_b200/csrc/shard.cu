@@ -248,7 +248,7 @@ static int comm_buffers(agb_comm *c, uint64_t local_cap, uint64_t pad_cap)
 static int shard_scan_geom(const agb_desc &d, const void *d_shard, uint64_t n_local, uint64_t halo_left, uint64_t halo_right,
                            bool first, bool open_end, bool reaches_end, int want, int want_level,
                            agb_record *d_records, uint64_t capacity, cudaStream_t st, agb_result *lres, agb_shard_part *part,
-                           const agb_regex *rx = nullptr, bool grow = false)
+                           const agb_pattern *px = nullptr, bool grow = false)
 {
 	if (((uintptr_t)d_shard & 15) || (halo_left & 15)) { snprintf(g_err, sizeof g_err, "shard pointer and left halo must be 16-byte aligned"); return AGB_ERR_ARG; }
 	if ((!first && (halo_left % 512)) || (!open_end && ((halo_left + n_local) % 512))) { snprintf(g_err, sizeof g_err, "shard boundaries must fall on multiples of 512 bytes of the scanned range"); return AGB_ERR_ARG; }
@@ -258,7 +258,7 @@ static int shard_scan_geom(const agb_desc &d, const void *d_shard, uint64_t n_lo
 	sh.own_lo = first ? INT64_MIN : (int64_t)halo_left;
 	sh.own_hi = open_end ? INT64_MAX : (int64_t)(halo_left + n_local);
 	sh.last = reaches_end ? 1 : 0;
-	int rc = scan_device_impl(d, text, n, want, want_level, d_records, (want & AGB_WANT_RECORDS) ? capacity : 0, st, lres, &sh, rx);
+	int rc = scan_device_impl(d, text, n, want, want_level, d_records, (want & AGB_WANT_RECORDS) ? capacity : 0, st, lres, &sh, px);
 	if (rc) return rc;
 	memset(part, 0, sizeof *part);
 	int dev = 0; CUDA_TRY(cudaGetDevice(&dev));
@@ -285,12 +285,12 @@ static int shard_scan_geom(const agb_desc &d, const void *d_shard, uint64_t n_lo
 
 /* one window of the windowed scan (scan.cu, scan_windowed): the shard scan in grow mode, then the window's records made
  * global on the device -- begin/end += byte_add, ordinal += ord_add -- by the gather kernel over a world of one */
-int shard_window_scan(const agb_desc &d, const agb_regex *rx, const void *d_win, uint64_t n_local, uint64_t halo_left, uint64_t halo_right,
+int shard_window_scan(const agb_desc &d, const agb_pattern *px, const void *d_win, uint64_t n_local, uint64_t halo_left, uint64_t halo_right,
                       bool first, bool open_end, bool reaches_end, int want, agb_record *d_records, uint64_t capacity,
                       cudaStream_t st, agb_result *lres, agb_shard_part *part)
 {
 	return shard_scan_geom(d, d_win, n_local, halo_left, halo_right, first, open_end, reaches_end, want, -1, d_records, capacity, st,
-	                       lres, part, rx, true);
+	                       lres, part, px, true);
 }
 
 int shard_window_rebase(agb_record *d_records, uint64_t n, long long byte_add, long long ord_add, bool ordinals, cudaStream_t st)
@@ -311,18 +311,18 @@ extern "C" int agb_scan_shard_local(const agb_pattern *p, const void *d_shard, u
 	if (!p || !res || !part) return AGB_ERR_ARG;
 	if ((want & AGB_WANT_RECORDS) && capacity && !d_records) return AGB_ERR_ARG;
 	return shard_scan_geom(p->d, d_shard, n_local, halo_left, halo_right, first != 0, open_end != 0, reaches_end != 0, want, -1,
-	                       d_records, capacity, (cudaStream_t)stream, res, part, agb_pattern_regex(p));
+	                       d_records, capacity, (cudaStream_t)stream, res, part, p);
 }
 
 /* this rank's part of a sharded scan; fills its header */
 static int shard_local_scan(const agb_desc &d, agb_comm *c, const void *d_shard, uint64_t n_local, int want, int want_level,
-                            uint64_t local_cap, cudaStream_t st, agb_result *lres, const agb_regex *rx = nullptr)
+                            uint64_t local_cap, cudaStream_t st, agb_result *lres, const agb_pattern *px = nullptr)
 {
 	if (!c->halo_known || c->sizes[c->rank] != n_local) { snprintf(g_err, sizeof g_err, "agb_shard_halo() has not been called for this shard"); return AGB_ERR_ARG; }
 	int rc = comm_buffers(c, (want & AGB_WANT_RECORDS) ? local_cap : 0, 0); if (rc) return rc;
 	agb_shard_part part;
 	rc = shard_scan_geom(d, d_shard, n_local, c->halo_left, c->halo_right, c->rank == 0, c->rank + 1 >= c->world, c->reaches_end != 0,
-	                     want, want_level, c->d_local, local_cap, st, lres, &part, rx);
+	                     want, want_level, c->d_local, local_cap, st, lres, &part, px);
 	if (rc) return rc;
 	unsigned long long *h = c->h_hdr;
 	memset(h, 0, HDR_WORDS * sizeof *h);
@@ -400,7 +400,7 @@ extern "C" int agb_scan_sharded(const agb_pattern *p, agb_comm *c, const void *d
 	CUDA_TRY(cudaSetDevice(c->dev));
 	agb_result lres;
 	/* a rank's own list can be as long as the whole capacity (all the matches may sit in one shard) */
-	int rc = shard_local_scan(p->d, c, d_shard, n_local, want, -1, capacity, st, &lres, agb_pattern_regex(p)); if (rc) return rc;
+	int rc = shard_local_scan(p->d, c, d_shard, n_local, want, -1, capacity, st, &lres, p); if (rc) return rc;
 	rc = shard_headers(c, st, res); if (rc) return rc;
 	if ((want & AGB_WANT_RECORDS) && capacity) { rc = shard_gather_lists(c, global_offset, want, d_records, capacity, st, res); if (rc) return rc; }
 	return AGB_OK;

@@ -321,9 +321,9 @@ int launch_slices(const agb_desc &d, const RecParams &P, unsigned grid, cudaStre
 	return narrow ? launch_slices_t<uint32_t, false>(d.nrows, P, grid, st) : launch_slices_t<uint64_t, false>(d.nrows, P, grid, st);
 }
 /* the slices form needs a bounded memory: no position that holds for ever ('#': wildmask; -p: Init1 = ~0) and a
- * delimiter whose occurrences do not depend on where a run of it started */
+ * delimiter whose occurrences do not depend on where a run of it started; and rows of at most 64 bits */
 bool slices_usable(const agb_desc &d)
 {
-	return d.wildmask == 0 && d.init1 != ~0ull && (d.L == 1 || d.delim_kind == 0) && d.M + d.nrows + 2 <= SL_APRON;
+	return !d.wide && d.wildmask == 0 && d.init1 != ~0ull && (d.L == 1 || d.delim_kind == 0) && d.M + d.nrows + 2 <= SL_APRON;
 }
 

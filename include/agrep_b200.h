@@ -103,7 +103,9 @@ typedef struct agb_desc {
 	/* 1: the anchors are the k + 2 equal-length pieces of the pair plan -- stage 1 flags a chunk only where one piece starts
 	 * and another one starts in it or in the chunk after it (set by the device scan's planner only; 0 from every caller) */
 	uint8_t  pair_plan;
-	uint8_t  pad_[1];
+	/* 1: the automaton's rows are 320 bits wide and its words are in agb_pattern_wide(), not here (set by agb_compile only;
+	 * 0 from every caller) */
+	uint8_t  wide;
 } agb_desc;
 
 typedef struct agb_pattern agb_pattern;       /* opaque: agb_desc + bookkeeping              */
@@ -121,6 +123,22 @@ typedef struct agb_regex {
 	int32_t  head, tail;                      /* HEAD / TAIL of preprocess(); tail: the epsilon move at '\n' (agrep.c:1332) */
 	int32_t  pad[2];
 } agb_regex;
+
+/* What a simple literal of more than 63 positions adds to the descriptor (AGB_ENGINE_SGREP_BM, k = 0: sgrep()'s bm() and
+ * monkey(), up to 255 characters as the reference accepts them, agrep.c:3057): the words of 320-bit rows.  Word 0 holds bits
+ * 0..63 of a row; position p is bit M-p, the always-on feed is bit M, as in the descriptor.  Masks that the descriptor
+ * fills "everywhere but" (init0's feed, noerr, dmask) are filled up to the end of the last word that holds bit M, and the
+ * words above it are zero, so a pattern of at most 63 positions has exactly its 64-bit words in word 0.  The descriptor of
+ * such a pattern has wide = 1, k = 0, nrows = 1, its real M and everything that is not a word (L, delim, delim_fold,
+ * delim_kind, engine, plan, anchors, pat_len, start_closes, inverse, user_delim, outtail); its 64-bit word fields (mask,
+ * init0 ... wildmask, reset, start) are zero. */
+#define AGB_WIDE_WORDS  5
+#define AGB_WIDE_MAXPOS (64 * AGB_WIDE_WORDS - 1)
+typedef struct agb_wide {
+	uint64_t mask[256][AGB_WIDE_WORDS];
+	uint64_t init0[AGB_WIDE_WORDS], init1[AGB_WIDE_WORDS], noerr[AGB_WIDE_WORDS], endpos[AGB_WIDE_WORDS];
+	uint64_t dendpos[AGB_WIDE_WORDS], dmask[AGB_WIDE_WORDS], reset[AGB_WIDE_WORDS], start[AGB_WIDE_WORDS];
+} agb_wide;
 
 /* one matching record, in the reference's own terms (file offsets, not buffer indexes):
  *   begin   = offset of lasti: first byte of the delimiter that closed the previous record; -1 for the
@@ -165,6 +183,10 @@ int  agb_pattern_from_desc(const agb_desc *d, agb_pattern **out, char *err, size
  * from words produced elsewhere (d->engine must be AGB_ENGINE_REGEX; reset[] and start[] are derived here) */
 const agb_regex *agb_pattern_regex(const agb_pattern *p);
 int  agb_pattern_from_regex(const agb_desc *d, const agb_regex *rx, agb_pattern **out, char *err, size_t errlen);
+/* the 320-bit words of a simple literal of more than 63 positions (NULL for every other pattern).  agb_pattern_from_desc
+ * refuses such descriptors: the drop-in's sgrep() compiles from the pattern text.  With AGB_FORCE_WIDE=1 in the
+ * environment agb_compile gives every AGB_ENGINE_SGREP_BM pattern this form (tests compare the two forms with it). */
+const agb_wide *agb_pattern_wide(const agb_pattern *p);
 
 /* ---- device scan ----
  * d_text: device pointer, 16-byte aligned, readable up to the next 16-byte boundary after n.
