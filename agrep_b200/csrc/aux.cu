@@ -437,7 +437,7 @@ __global__ void __launch_bounds__(256) k_ordinals_set(const OrdParams P0, const 
 
 /* after stage 1: is the bitmap so full that thinning it (stage 1.5) and walking a candidate list cannot pay?  Then the
  * record stage walks every byte anyway (slices / dense tile form) and stage 1.5 is skipped.  Estimated from every
- * 61st bitmap word; same 5 % threshold as the list/dense switch in records_launch(). */
+ * 61st bitmap word, against the list form's threshold. */
 int front_is_dense(Workspace &W, uint64_t n, cudaStream_t st, bool *dense)
 {
 	const uint64_t n_chunks = (n + 15) / 16, n_words = (n_chunks + 31) / 32;
@@ -448,7 +448,7 @@ int front_is_dense(Workspace &W, uint64_t n, cudaStream_t st, bool *dense)
 	k_bitmap_sample<<<grid ? grid : 1, 256, 0, st>>>(W.bitmap, n_words, stride, W.totals + 14); g_launches++;
 	CUDA_TRY(cudaMemcpyAsync(W.h_totals + 14, W.totals + 14, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
 	CUDA_TRY(cudaStreamSynchronize(st));
-	*dense = W.h_totals[14] * stride > n_chunks / 20 + 1024;
+	*dense = !list_form_pays(W.h_totals[14] * stride, n_chunks);
 	return AGB_OK;
 }
 

@@ -2,34 +2,6 @@
  * instantiations for 32- and 64-bit rows, and the launchers of every row width */
 #include "records_kernel.cuh"
 
-template <typename T, bool COSTS>
-static int launch_records_t(int nrows, const RecParams &P, unsigned grid, cudaStream_t st)
-{
-	switch (nrows) {
-	case 1: k_records<T, 1, COSTS><<<grid, REC_THREADS, 0, st>>>(P); break;
-	case 2: k_records<T, 2, COSTS><<<grid, REC_THREADS, 0, st>>>(P); break;
-	case 3: k_records<T, 3, COSTS><<<grid, REC_THREADS, 0, st>>>(P); break;
-	case 4: k_records<T, 4, COSTS><<<grid, REC_THREADS, 0, st>>>(P); break;
-	case 5: k_records<T, 5, COSTS><<<grid, REC_THREADS, 0, st>>>(P); break;
-	case 6: k_records<T, 6, COSTS><<<grid, REC_THREADS, 0, st>>>(P); break;
-	case 7: k_records<T, 7, COSTS><<<grid, REC_THREADS, 0, st>>>(P); break;
-	case 8: k_records<T, 8, COSTS><<<grid, REC_THREADS, 0, st>>>(P); break;
-	case 9: k_records<T, 9, COSTS><<<grid, REC_THREADS, 0, st>>>(P); break;
-	default: return -1;
-	}
-	g_launches++;
-	return 0;
-}
-
-int launch_records(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st)
-{
-	if (d.wide) return launch_records_wide(P, grid, st);
-	bool costs = d.engine == AGB_ENGINE_ASEARCH1;
-	bool narrow = d.M <= 31;        /* the reference's own word width; wider patterns use 64-bit rows */
-	if (costs) return narrow ? launch_records_t<uint32_t, true>(d.nrows, P, grid, st) : launch_records_t<uint64_t, true>(d.nrows, P, grid, st);
-	return narrow ? launch_records_t<uint32_t, false>(d.nrows, P, grid, st) : launch_records_t<uint64_t, false>(d.nrows, P, grid, st);
-}
-
 template <typename T, bool COSTS, bool SET>
 static int launch_dense_t(int nrows, const RecParams &P, unsigned grid, cudaStream_t st)
 {

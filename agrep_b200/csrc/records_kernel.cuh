@@ -1,6 +1,6 @@
-/* agrep_b200/csrc/records_kernel.cuh -- stage 2, the forms that start from record boundaries: bitmap form (k_records),
- * dense tile form (k_records_dense), list form (k_records_list) (DESIGN.md 3.3).  Instantiated by records.cu (32- and
- * 64-bit rows) and records_wide.cu (320-bit rows) */
+/* agrep_b200/csrc/records_kernel.cuh -- stage 2, the forms that start from record boundaries: dense tile form
+ * (k_records_dense), list form (k_records_list) (DESIGN.md 3.3).  Instantiated by records.cu (32- and 64-bit rows) and
+ * records_wide.cu (320-bit rows) */
 #ifndef AGB_RECORDS_KERNEL_CUH
 #define AGB_RECORDS_KERNEL_CUH
 #include "automaton.cuh"
@@ -10,39 +10,31 @@
  * stage 2: records
  * ============================================================================================== */
 
-/* The records chunk c owns: a record [s-1, close) belongs to the FIRST flagged chunk that meets it, so
- *   (a) the record that contains byte 16c is ours iff its re-fed byte s-1 lies after the previous flagged chunk
- *       (search backwards, stop at a delimiter end -> ours, or at a flagged chunk -> theirs);
+/* The records candidate chunk c owns: a record [s-1, close) belongs to the FIRST flagged chunk that meets it, so
+ *   (a) the record that contains byte 16c is ours iff its re-fed byte s-1 lies after prev, the flagged chunk before c
+ *       (search backwards, stop at a delimiter end -> ours, or at prev -> theirs);
  *   (b) every record whose re-fed byte lies inside the chunk is ours.
- * done_until (dense form) remembers how far this thread's previous chunk already got.
  * Returns the number of reported records; writes them at out_pos.. when write is set. */
 template <typename T, int NR, bool COSTS, typename RD>
 __device__ __forceinline__ uint32_t chunk_records(const RecParams &P, const DevConsts<T> &C, RecShared<T, NR> &SH, RD &R,
-                                                 const int64_t c, int64_t &done_until, const bool write, const uint64_t out_pos, const bool hist,
-                                                 agb_record *first_out = nullptr, const int64_t prev_flagged = -2)
+                                                 const int64_t c, const bool write, const uint64_t out_pos, const bool hist,
+                                                 agb_record *first_out, const int64_t prev)
 {
 	const int L = C.L;
 	const int64_t n = (int64_t)P.n, lo = c * 16, hi = lo + 15;
 	uint32_t cnt = 0;
 	int64_t s = -2;                /* record start to run from; -2: none */
-	if (done_until > lo) {
-		/* the record this thread closed last reaches into this chunk; what starts here starts at done_until */
-		if (done_until - 1 <= hi) s = done_until; else return 0;
-	} else {
-		bool found = false;
-		if (c == 0) { s = 0; found = true; }
-		for (int64_t cc = c - 1; !found; cc--) {
-			if (cc < 0) { s = 0; found = true; break; }
-			/* an earlier flagged chunk meets that record: not ours (list form: the flagged chunk before c is known) */
-			if (prev_flagged != -2) { if (cc == prev_flagged) break; }
-			else { const uint32_t pw = P.bitmap ? P.bitmap[cc >> 5] : 0xffffffffu; if (pw >> (cc & 31) & 1u) break; }
-			for (int64_t q = cc * 16 + 15; q >= cc * 16; q--)
-				if (delim_ends_at(R, q, SH.delim, SH.dfold, L, C.kind)) { s = q + 1; found = true; break; }
-		}
-		if (!found) {
-			for (int64_t q = lo; q <= hi && q < n; q++)
-				if (delim_ends_at(R, q, SH.delim, SH.dfold, L, C.kind)) { s = q + 1; break; }
-		}
+	bool found = false;
+	if (c == 0) { s = 0; found = true; }
+	for (int64_t cc = c - 1; !found; cc--) {
+		if (cc < 0) { s = 0; found = true; break; }
+		if (cc == prev) break;     /* an earlier flagged chunk meets that record: not ours */
+		for (int64_t q = cc * 16 + 15; q >= cc * 16; q--)
+			if (delim_ends_at(R, q, SH.delim, SH.dfold, L, C.kind)) { s = q + 1; found = true; break; }
+	}
+	if (!found) {
+		for (int64_t q = lo; q <= hi && q < n; q++)
+			if (delim_ends_at(R, q, SH.delim, SH.dfold, L, C.kind)) { s = q + 1; break; }
 	}
 	/* run records while their re-fed byte (s-1) is at or before the end of this chunk */
 	while (s >= 0 && s - 1 <= hi && s <= n) {
@@ -63,7 +55,7 @@ __device__ __forceinline__ uint32_t chunk_records(const RecParams &P, const DevC
 			rows_step<T, NR, COSTS>(S, SH.mask[R.get(p)], C);
 			if (S[0] & C.dendpos) { close_at = p; break; }
 		}
-		if (close_at < 0) { done_until = limit + 1; break; }           /* never closed: dropped, as the reference does */
+		if (close_at < 0) break;                                      /* never closed: dropped, as the reference does */
 		const int64_t end = close_at + 1 - L;
 		const bool counts = (begin + 1 < n) && (begin + 1 <= end) && rec_owned(P, begin, L, close_at);       /* bitap.c:213 + agrep.c:3811 */
 		int level = C.k;
@@ -88,62 +80,8 @@ __device__ __forceinline__ uint32_t chunk_records(const RecParams &P, const DevC
 			cnt++;
 		}
 		s = close_at + 1;
-		done_until = s;
 	}
 	return cnt;
-}
-
-/* dense form: every thread owns one bitmap word (32 chunks); used when the plan flags everything or stage 1.5
- * cannot thin the bitmap.  Count pass -> per-tile counts; emit pass recounts, scans inside the block, writes. */
-template <typename T, int NR, bool COSTS>
-__global__ void __launch_bounds__(REC_THREADS)
-k_records(const RecParams P)
-{
-	__shared__ RecShared<T, NR> SH;
-	__shared__ uint32_t s_scan[REC_THREADS];
-	DevConsts<T> C;
-	shared_init<T, NR>(SH, C, P.desc, REC_THREADS, P.rx_tab);
-	const uint64_t gw = (uint64_t)blockIdx.x * REC_THREADS + threadIdx.x;     /* bitmap word of this thread */
-	uint32_t word = 0;
-	if (gw < P.n_words) {
-		word = P.bitmap ? P.bitmap[gw] : 0xffffffffu;
-		uint64_t rem = P.n_chunks - gw * 32;
-		if (rem < 32) word &= (1u << rem) - 1u;
-	}
-	Reader R; R.init(P.text, P.n, SH.delim, C.L);
-	uint32_t my_count = 0;
-	uint64_t out_pos = 0;
-	for (int pass = 0; pass < (P.emit ? 2 : 1); pass++) {
-		uint32_t bits = word, cnt = 0;
-		int64_t done_until = INT64_MIN;
-		while (bits) {
-			const int b = __ffs(bits) - 1; bits &= bits - 1;
-			cnt += chunk_records<T, NR, COSTS>(P, C, SH, R, (int64_t)(gw * 32 + b), done_until, pass == 1, out_pos + cnt, pass == 0 && !P.emit);
-		}
-		if (pass == 0) {
-			my_count = cnt;
-			s_scan[threadIdx.x] = cnt;
-			__syncthreads();
-			for (int off = 1; off < REC_THREADS; off <<= 1) {
-				uint32_t v = (threadIdx.x >= (unsigned)off) ? s_scan[threadIdx.x - off] : 0;
-				__syncthreads();
-				s_scan[threadIdx.x] += v;
-				__syncthreads();
-			}
-			if (!P.emit) {
-				if (threadIdx.x == REC_THREADS - 1) {
-					P.tile_counts[blockIdx.x] = s_scan[REC_THREADS - 1];
-					if (s_scan[REC_THREADS - 1]) atomicAdd(&P.totals[0], (unsigned long long)s_scan[REC_THREADS - 1]);
-				}
-				uint32_t fl = __reduce_add_sync(0xffffffffu, (uint32_t)__popc(word));
-				if ((threadIdx.x & 31) == 0 && fl) atomicAdd(&P.totals[1], (unsigned long long)fl);
-				__syncthreads();
-				if (P.levels && threadIdx.x <= AGB_MAXERR && SH.hist[threadIdx.x]) atomicAdd(&P.totals[2 + threadIdx.x], SH.hist[threadIdx.x]);
-			} else {
-				out_pos = P.tile_offsets[blockIdx.x] + (s_scan[threadIdx.x] - my_count);
-			}
-		}
-	}
 }
 
 /* dense tile form: the automaton over EVERYTHING (no anchor plan: classes, -v, -p, '#', short patterns ...).
@@ -421,10 +359,9 @@ k_records_list(const RecParams P)
 			if (hi > (int64_t)P.n) hi = (int64_t)P.n;          /* only bytes of the text (the slow path knows the virtual and appended ones) */
 			R.sm = reinterpret_cast<const uint8_t *>(strip); R.lo = g0 * 16; R.len = (uint32_t)(hi - g0 * 16);
 		}
-		int64_t done_until = INT64_MIN;
-		if (P.emit) chunk_records<T, NR, COSTS>(P, C, SH, R, c, done_until, true, P.tile_offsets[i], false, nullptr, prev);
+		if (P.emit) chunk_records<T, NR, COSTS>(P, C, SH, R, c, true, P.tile_offsets[i], false, nullptr, prev);
 		else {
-			const uint32_t c1 = chunk_records<T, NR, COSTS>(P, C, SH, R, c, done_until, false, 0, true, P.cand_first ? &P.cand_first[i] : nullptr, prev);
+			const uint32_t c1 = chunk_records<T, NR, COSTS>(P, C, SH, R, c, false, 0, true, P.cand_first ? &P.cand_first[i] : nullptr, prev);
 			P.tile_counts[i] = c1;
 			cnt += c1;
 		}

@@ -1,13 +1,7 @@
 /* agrep_b200/csrc/records_wide.cu -- stage 2 for 320-bit rows: simple literals of more than 63 positions at k = 0
- * (agb_wide).  The forms of records_kernel.cuh at one row; there is no slices form for them (slices_usable). */
+ * (agb_wide).  The dense tile and list forms of records_kernel.cuh at one row; there is no slices form for them
+ * (slices_usable). */
 #include "records_kernel.cuh"
-
-int launch_records_wide(const RecParams &P, unsigned grid, cudaStream_t st)
-{
-	k_records<Wide, 1, false><<<grid, REC_THREADS, 0, st>>>(P);
-	g_launches++;
-	return 0;
-}
 
 int launch_dense_wide(const RecParams &P, unsigned grid, cudaStream_t st, bool set)
 {

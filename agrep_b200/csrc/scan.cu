@@ -8,10 +8,11 @@
  *              anchors starts there (pigeonhole, pattern.c:plan_anchors); one bit per chunk.  HBM-bound.
  *   stage 1.5  k_refine (refine.cu)  the same recurrence over just the window around an anchor hit; chunks whose
  *              hits cannot belong to a match lose their bit.
- *   stage 2    records (records.cu, slices.cu)  exact: the recurrence from the record start in the constant
+ *   stage 2    records (records.cu, slices.cu, regex.cu)  exact: the recurrence from the record start in the constant
  *              post-delimiter state until the closing delimiter, the reference's match test and bookkeeping,
- *              ordered (lasti, print_end) lists by count pass -> scan -> emit pass.  List form for sparse
- *              survivors, slices / dense tile form when every byte has to be walked.
+ *              ordered (lasti, print_end) lists by count pass -> scan -> emit pass.  The list form for the flagged
+ *              chunks while they are sparse; the slices or dense tile form when every byte has to be walked; k_regex
+ *              for regular expressions.
  *   ordinals   (aux.cu)  the j that -n prints, from delimiter counts.
  *
  * This file: the per-device workspace, which form runs when (records_launch), the streaming host entry points
@@ -185,92 +186,78 @@ static int list_stage(const agb_desc &d, Workspace &W, RecParams &P, bool want_l
 	return AGB_OK;
 }
 
-/* stage 2 over the whole text.  After stage 1.5 the survivors are few: they are compacted into an ordered list
- * and each gets its own thread (count launch -> scan -> emit launch).  Otherwise (or if the list would not fit)
- * the dense form walks the bitmap, one thread per word.
- * refined: stage 1.5 ran -- the survivors are in W.bitmap2, their per-range counts in W.range_counts, and nothing
- * here needs the host to know how many there are (the list is sized by W.cand_hint / a fraction of the chunks; the
- * caller, stages_after_front, reads totals[12] back and, if it exceeds W.cand_cap, calls this again -- with the list
- * sized from that count, or with use_front off for the every-byte form when the survivors are dense). */
-static int records_launch(const agb_desc &d, Workspace &W, const void *d_text, uint64_t n, bool use_front, bool refined, int want,
+/* a tile form (launch_slices, launch_dense, launch_regex and their SET forms) -> records: count launch (per-tile counts),
+ * scan, emit launch, one block per tile */
+typedef int (*TileLaunch)(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
+static int tile_stage(TileLaunch launch, const agb_desc &d, RecParams &P, Workspace &W, unsigned grid, bool want_list, cudaStream_t st)
+{
+	P.tile_counts = W.tile_counts; P.tile_offsets = W.tile_offsets;
+	if (launch(d, P, grid, st)) return AGB_ERR_ARG;
+	CUDA_TRY(cudaGetLastError());
+	if (want_list) {
+		k_scan_tiles<<<1, 1024, 0, st>>>(W.tile_counts, W.tile_offsets, grid, nullptr); g_launches++;
+		P.emit = 1;
+		if (launch(d, P, grid, st)) return AGB_ERR_ARG;
+		CUDA_TRY(cudaGetLastError());
+	}
+	return AGB_OK;
+}
+
+/* what feeds the record stage */
+enum RecInput {
+	REC_EVERY_BYTE,              /* no bitmap: every byte is walked */
+	REC_FRONT,                   /* stage 1's bitmap (W.bitmap), for the patterns stage 1.5 cannot thin (refine_launch) */
+	REC_SURVIVORS,               /* stage 1.5's survivors (W.bitmap2), their per-range counts in W.range_counts */
+};
+
+/* stage 2 over the whole text.  Regular expressions: k_regex over every byte.  Otherwise, by input:
+ *   REC_SURVIVORS   compacted into the ordered candidate list, then the list form.  The list is sized without asking the
+ *                   device how many survivors there are (W.cand_hint, or a fraction of the chunks); the caller,
+ *                   stages_after_front, reads totals[12] back and, if it exceeds W.cand_cap, calls this again -- with the
+ *                   list sized from that count, or with REC_EVERY_BYTE when the survivors are dense.
+ *   REC_FRONT       the flagged chunks are counted and the count read back: the list form while list_form_pays, else
+ *                   every byte.
+ *   REC_EVERY_BYTE  the slices form, or the dense tile form for the patterns slices_usable turns away. */
+static int records_launch(const agb_desc &d, Workspace &W, const void *d_text, uint64_t n, RecInput in, int want,
                           int want_level, agb_record *d_records, uint64_t capacity, cudaStream_t st, const ShardInfo *sh)
 {
-	const uint64_t n_chunks = (n + 15) / 16, n_words = (n_chunks + 31) / 32, tiles = (n_words + REC_THREADS - 1) / REC_THREADS;
+	const uint64_t n_chunks = (n + 15) / 16;
 	RecParams P; memset(&P, 0, sizeof P);
-	P.text = (const uint8_t *)d_text; P.bitmap = use_front ? (refined ? W.bitmap2 : W.bitmap) : nullptr;
-	P.n = n; P.n_chunks = n_chunks; P.n_words = n_words; P.desc = W.d_desc;
+	P.text = (const uint8_t *)d_text; P.n = n; P.n_chunks = n_chunks; P.desc = W.d_desc;
 	P.records = d_records; P.capacity = capacity;
 	P.totals = W.totals; P.emit = 0; P.levels = (want & AGB_WANT_LEVELS) ? 1 : 0; P.want_level = want_level;
 	P.own_lo = sh ? sh->own_lo : INT64_MIN; P.own_hi = sh ? sh->own_hi : INT64_MAX; P.shard_last = sh ? sh->last : 1;
 	P.rx_tab = W.d_regex; P.rx_tail = W.regex_tail;
-	if (!tiles) return AGB_OK;
+	if (!n) return AGB_OK;
 	const bool want_list = (want & AGB_WANT_RECORDS) && capacity;
-	if (d.engine == AGB_ENGINE_REGEX) {
-		/* regular expressions: no anchor plan, every byte through re()'s recurrence in the tile form (regex.cu) */
-		P.tile_counts = W.tile_counts; P.tile_offsets = W.tile_offsets;
-		const uint64_t rtiles = (n + DENSE_TILE - 1) / DENSE_TILE;
-		if (launch_regex(d, P, (unsigned)rtiles, st)) return AGB_ERR_ARG;
-		CUDA_TRY(cudaGetLastError());
-		if (want_list) {
-			k_scan_tiles<<<1, 1024, 0, st>>>(W.tile_counts, W.tile_offsets, rtiles, nullptr); g_launches++;
-			P.emit = 1;
-			if (launch_regex(d, P, (unsigned)rtiles, st)) return AGB_ERR_ARG;
-			CUDA_TRY(cudaGetLastError());
-		}
-		return AGB_OK;
-	}
-	if (use_front && refined) {
+	if (d.engine == AGB_ENGINE_REGEX)
+		return tile_stage(launch_regex, d, P, W, (unsigned)((n + RX_TILE - 1) / RX_TILE), want_list, st);
+	if (in == REC_SURVIVORS) {
 		int rc = ws_cand_reserve(W, std::max<size_t>(W.cand_hint + W.cand_hint / 4, (size_t)(n_chunks / 512) + 65536)); if (rc) return rc;
 		const unsigned ranges = W.refine_ctas * (REFINE_THREADS / 32);
 		k_scan_tiles<<<1, 1024, 0, st>>>(W.range_counts, W.range_offsets, ranges, W.totals + 12); g_launches++;
 		rc = compact_ranges_launch(W, n, st); if (rc) return rc;
 		return list_stage(d, W, P, want_list, st);
 	}
-	if (use_front) {
-		const uint64_t blocks = (n_words + COMPACT_THREADS * COMPACT_WPT - 1) / (COMPACT_THREADS * COMPACT_WPT);
+	if (in == REC_FRONT) {
+		const uint64_t n_words = (n_chunks + 31) / 32, blocks = (n_words + COMPACT_THREADS * COMPACT_WPT - 1) / (COMPACT_THREADS * COMPACT_WPT);
 		k_compact_count<<<(unsigned)blocks, COMPACT_THREADS, 0, st>>>(W.bitmap, n_words, W.tile_counts, W.totals); g_launches++;
 		k_scan_tiles<<<1, 1024, 0, st>>>(W.tile_counts, W.tile_offsets, blocks, W.totals + 12); g_launches++;
 		CUDA_TRY(cudaMemcpyAsync(W.h_totals + 12, W.totals + 12, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
 		CUDA_TRY(cudaStreamSynchronize(st));
 		const unsigned long long ncand = W.h_totals[12];
-		/* list form while the survivors are sparse (20 B of scratch each): one thread per candidate against the dense
-		 * tile kernel's walk over every byte; the cross-over is put at 5 % of the chunks ('the' flags 11 %, 'government' 1.1 %) */
-		const bool sparse = ncand <= n_chunks / 20 + 1024;
-		if (!sparse) {
-			CUDA_TRY(cudaMemsetAsync(W.totals + 1, 0, sizeof(unsigned long long), st));
-			use_front = false; P.bitmap = nullptr;
-		} else if (ws_cand_reserve(W, (size_t)ncand) == AGB_OK) {
+		if (list_form_pays(ncand, n_chunks)) {
+			int rc = ws_cand_reserve(W, (size_t)ncand); if (rc) return rc;
 			if (ncand == 0) return AGB_OK;
 			k_compact_write<<<(unsigned)blocks, COMPACT_THREADS, 0, st>>>(W.bitmap, n_words, W.tile_offsets, W.cand, W.cand_cap); g_launches++;
 			return list_stage(d, W, P, want_list, st);
 		}
-		else CUDA_TRY(cudaMemsetAsync(W.totals + 1, 0, sizeof(unsigned long long), st));   /* no scratch for a list: bitmap form below recounts totals[1] */
+		CUDA_TRY(cudaMemsetAsync(W.totals + 1, 0, sizeof(unsigned long long), st));   /* the tile form counts totals[1] afresh */
 	}
-	P.tile_counts = W.tile_counts; P.tile_offsets = W.tile_offsets;
-	if (!use_front) {
-		/* no bitmap at all: the dense tile kernel, one CTA per 32 KiB (tile_counts has n/64KiB... entries: 2 per REC tile) */
-		const bool slices = slices_usable(d);
-		const uint64_t dtiles = slices ? (n + SL_TILE - 1) / SL_TILE : (n + DENSE_TILE - 1) / DENSE_TILE;
-		P.warm = (d.M + d.nrows + 2 + 3) & ~3;
-		if (slices ? launch_slices(d, P, (unsigned)dtiles, st) : launch_dense(d, P, (unsigned)dtiles, st)) return AGB_ERR_ARG;
-		CUDA_TRY(cudaGetLastError());
-		if (want_list) {
-			k_scan_tiles<<<1, 1024, 0, st>>>(W.tile_counts, W.tile_offsets, dtiles, nullptr); g_launches++;
-			P.emit = 1;
-			if (slices ? launch_slices(d, P, (unsigned)dtiles, st) : launch_dense(d, P, (unsigned)dtiles, st)) return AGB_ERR_ARG;
-			CUDA_TRY(cudaGetLastError());
-		}
-		return AGB_OK;
-	}
-	if (launch_records(d, P, (unsigned)tiles, st)) return AGB_ERR_ARG;
-	CUDA_TRY(cudaGetLastError());
-	if (want_list) {
-		k_scan_tiles<<<1, 1024, 0, st>>>(W.tile_counts, W.tile_offsets, tiles, nullptr); g_launches++;
-		P.emit = 1;
-		if (launch_records(d, P, (unsigned)tiles, st)) return AGB_ERR_ARG;
-		CUDA_TRY(cudaGetLastError());
-	}
-	return AGB_OK;
+	const bool slices = slices_usable(d);
+	P.warm = (d.M + d.nrows + 2 + 3) & ~3;
+	return tile_stage(slices ? launch_slices : launch_dense, d, P, W,
+	                  (unsigned)(slices ? (n + SL_TILE - 1) / SL_TILE : (n + DENSE_TILE - 1) / DENSE_TILE), want_list, st);
 }
 
 /* an exact pattern that is no longer than its anchor ('the'): every chunk stage 1 flags holds a real occurrence, so
@@ -522,21 +509,21 @@ static int stages_after_front(const agb_desc &d, Workspace &W, const void *d_tex
 {
 	int rc;
 	const uint64_t n_chunks = (n + 15) / 16;
-	if (use_front && refine_cannot_thin(d)) { bool dense = false; rc = front_is_dense(W, n, st, &dense); if (rc) return rc; if (dense) use_front = false; }
-	bool refined = false;
-	if (use_front) { rc = refine_launch(d, W, d_text, n, st, &refined); if (rc) return rc; }
+	RecInput in = use_front ? REC_FRONT : REC_EVERY_BYTE;
+	if (in == REC_FRONT && refine_cannot_thin(d)) { bool dense = false; rc = front_is_dense(W, n, st, &dense); if (rc) return rc; if (dense) in = REC_EVERY_BYTE; }
+	if (in == REC_FRONT) { bool refined = false; rc = refine_launch(d, W, d_text, n, st, &refined); if (rc) return rc; if (refined) in = REC_SURVIVORS; }
 	for (int attempt = 0; ; attempt++) {
-		rc = records_launch(d, W, d_text, n, use_front, refined, want, want_level, d_records, capacity, st, sh); if (rc) return rc;
+		rc = records_launch(d, W, d_text, n, in, want, want_level, d_records, capacity, st, sh); if (rc) return rc;
 		if (want & AGB_WANT_ORDINALS) { rc = ordinals_launch(d, W, d_text, n, (want & AGB_WANT_RECORDS) ? d_records : nullptr, capacity, st, count_in_front); if (rc) return rc; }
 		CUDA_TRY(cudaEventRecord(W.e2, st));
 		if (sh) { rc = shard_aux_enqueue(d, W, (const uint8_t *)d_text, n, sh, (want & AGB_WANT_ORDINALS) != 0, st); if (rc) return rc; }
-		rc = fetch_result(W, want, capacity, use_front && refined, st, res); if (rc) return rc;
-		if (!(use_front && refined)) break;
+		rc = fetch_result(W, want, capacity, in == REC_SURVIVORS, st, res); if (rc) return rc;
+		if (in != REC_SURVIVORS) break;
 		const uint64_t ncand = W.h_totals[12];
 		W.cand_hint = (size_t)ncand;
 		if (ncand <= W.cand_cap || attempt) break;
 		/* the list was too small: again, with the size known now (sparse) or over every byte (dense) */
-		if (ncand > n_chunks / 20 + 1024) { use_front = false; refined = false; }
+		if (!list_form_pays(ncand, n_chunks)) in = REC_EVERY_BYTE;
 		CUDA_TRY(cudaMemsetAsync(W.totals, 0, 12 * sizeof(unsigned long long), st));
 	}
 	return AGB_OK;
@@ -1158,19 +1145,10 @@ extern "C" int agb_scan_set(const agb_pattern *p, const void *const *h_texts, co
 	P.levels = (want & AGB_WANT_LEVELS) ? 1 : 0; P.want_level = -1;
 	P.own_lo = INT64_MIN; P.own_hi = INT64_MAX; P.shard_last = 1;
 	P.rx_tab = W.d_regex; P.rx_tail = W.regex_tail;
-	P.tile_counts = W.tile_counts; P.tile_offsets = W.tile_offsets;
 	P.set_files = d_files; P.set_tiles = d_rtiles; P.set_stats = d_stats;
-	const bool regex = d.engine == AGB_ENGINE_REGEX;
-	const unsigned grid = (unsigned)rtiles.size();
-	if (grid) {
-		if (regex ? launch_regex_set(d, P, grid, H.s_comp) : launch_dense_set(d, P, grid, H.s_comp)) return AGB_ERR_ARG;
-		CUDA_TRY(cudaGetLastError());
-		if (want_list) {
-			k_scan_tiles<<<1, 1024, 0, H.s_comp>>>(W.tile_counts, W.tile_offsets, grid, nullptr); g_launches++;
-			P.emit = 1;
-			if (regex ? launch_regex_set(d, P, grid, H.s_comp) : launch_dense_set(d, P, grid, H.s_comp)) return AGB_ERR_ARG;
-			CUDA_TRY(cudaGetLastError());
-		}
+	if (!rtiles.empty()) {
+		rc = tile_stage(d.engine == AGB_ENGINE_REGEX ? launch_regex_set : launch_dense_set, d, P, W, (unsigned)rtiles.size(), want_list, H.s_comp);
+		if (rc) return rc;
 	}
 	if (ord) { rc = ordinals_set_launch(d, W, H.text, d_files, d_otiles, otiles.size(), d_stats, want_list ? H.rec : nullptr, list_cap, H.s_comp); if (rc) return rc; }
 	CUDA_TRY(cudaEventRecord(W.e2, H.s_comp));

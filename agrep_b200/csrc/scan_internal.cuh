@@ -2,7 +2,7 @@
  * geometry, kernel parameter blocks, the per-device workspace and the host functions that cross files.
  *   front.cu    stage 1   k_front            (anchor filter, HBM-bound)
  *   refine.cu   stage 1.5 k_refine           (local verification of anchor hits)
- *   records.cu  stage 2   k_records, k_records_dense, k_records_list (records_kernel.cuh; records_wide.cu: 320-bit rows)
+ *   records.cu  stage 2   k_records_dense, k_records_list (records_kernel.cuh; records_wide.cu: 320-bit rows)
  *   slices.cu   stage 2   k_records_slices   (the automaton over every byte, in lockstep)
  *   regex.cu    stage 2   k_regex            (regular expressions: re()'s recurrence over every byte, tile form)
  *   aux.cu      bitmap compaction, scans, density sample, ordinals, synthetic corpus
@@ -80,12 +80,11 @@ struct RefineParams {
 };
 
 /* ---- stage 2 ---- */
-#define REC_THREADS 128          /* dense form: one thread per bitmap word, a block covers 128*512 B = 64 KiB of text */
+#define REC_THREADS 128          /* list form: threads per block, one candidate each */
 
 struct RecParams {
 	const uint8_t  *text;
-	const uint32_t *bitmap;      /* NULL: every chunk flagged */
-	uint64_t n, n_chunks, n_words;
+	uint64_t n, n_chunks;
 	const agb_desc *desc;        /* device copy */
 	uint32_t *tile_counts;       /* dense: per block; list: per candidate */
 	const uint64_t *tile_offsets;/* exclusive scan of tile_counts (emit pass) */
@@ -132,6 +131,9 @@ struct ShardInfo { int64_t own_lo, own_hi; int last; };
 #define COMPACT_THREADS 256
 #define COMPACT_WPT 4            /* words per thread: a block covers 1024 words */
 #define SCAN_BLOCK 16384
+/* the record stage's list form pays while at most 5 % of the chunks are flagged: one thread per candidate (20 B of
+ * scratch each) against a tile form's walk over every byte ('the' flags 11 % of the chunks, 'government' 1.1 %) */
+static inline bool list_form_pays(uint64_t flagged, uint64_t n_chunks) { return flagged <= n_chunks / 20 + 1024; }
 
 /* ---- ordinals ---- */
 #define ORD_THREADS 256
@@ -212,7 +214,6 @@ unsigned refine_grid(const Workspace &W, uint64_t n);
 int  compact_ranges_launch(Workspace &W, uint64_t n, cudaStream_t st);
 #define REFINE_MAX_RANGES 16384  /* >= warps of the largest stage 1.5 grid */
 /* records.cu, slices.cu: one launch of the given form (count pass or emit pass, RecParams.emit) */
-int  launch_records(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 int  launch_dense(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 /* the SET form of the dense tile kernel and of k_regex: one block per entry of P.set_tiles */
 int  launch_dense_set(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
@@ -220,7 +221,6 @@ int  launch_regex_set(const agb_desc &d, const RecParams &P, unsigned grid, cuda
 int  launch_records_list(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 /* records_wide.cu: the same forms for 320-bit rows (agb_desc.wide: the words in RecParams.rx_tab), which the launchers
  * above hand over to */
-int  launch_records_wide(const RecParams &P, unsigned grid, cudaStream_t st);
 int  launch_dense_wide(const RecParams &P, unsigned grid, cudaStream_t st, bool set);
 int  launch_records_list_wide(const RecParams &P, unsigned grid, cudaStream_t st);
 int  launch_slices(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);

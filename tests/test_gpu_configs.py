@@ -54,7 +54,9 @@ def test_the_record_stage_gets_few_chunks_when_the_filters_can_thin():
     """which form runs is a performance decision, not a parity one -- so it gets its own check: n_flagged is the number
     of chunks handed to the record stage.  Patterns of common words flag several per cent of the chunks in stage 1;
     stage 1.5 must still run and leave almost nothing (a shortcut that sent the k=4 case to the every-byte form cost
-    6x), while an exact short literal that is everywhere goes to the every-byte form directly."""
+    6x), while an exact short literal that is everywhere goes to the every-byte form directly.  A multi-part pattern has
+    no stage 1.5: stage 1's flags go to the list form while they are few ('gove' of the;government flags 1.1 %) and to
+    the every-byte form when they are not ('the' or 'gov' of the,government flags 12 %); both against the checker."""
     n = 16384 * PAGE                                  # 64 MiB
     host = ag.corpus_host(n, needle="because each", needle_every=4096, needle_maxedits=3)
     chunks = n // 16
@@ -64,6 +66,13 @@ def test_the_record_stage_gets_few_chunks_when_the_filters_can_thin():
         assert res.n_flagged < chunks // 20, (pat, kw, res.n_flagged, chunks)
     res, _ = ag.Pattern("the").scan_host(host, want_records=False)
     assert res.n_flagged == chunks
+    for pat, sparse in (("the;government", True), ("the,government", False)):
+        a = _oracle.compile(pat)
+        cnt, _ = _oracle.scan(a, host, want_records=False)
+        _, recs = _oracle.scan(a, host, cap=cnt)          # (the default room, a record per byte, is 1.6 GB here)
+        res, got = ag.Pattern(pat).scan_host(host)
+        assert res.n_matched == cnt and [(b, e) for b, e, _, _ in got] == [(b, e) for b, e, _ in recs], pat
+        assert (0 < res.n_flagged < chunks // 20) if sparse else res.n_flagged == chunks, (pat, res.n_flagged, chunks)
 
 
 def test_anchor_planner_plans_agree(monkeypatch):
