@@ -20,7 +20,7 @@ class Options(C.Structure):
     _fields_ = [("k", C.c_int32), ("nocase", C.c_int32), ("wordbound", C.c_int32), ("wholeline", C.c_int32),
                 ("inverse", C.c_int32), ("linenum", C.c_int32), ("ins_free", C.c_int32),
                 ("cost_i", C.c_int32), ("cost_s", C.c_int32), ("cost_d", C.c_int32),
-                ("bestmatch", C.c_int32), ("regex", C.c_int32), ("delim", C.c_char_p)]
+                ("bestmatch", C.c_int32), ("regex", C.c_int32), ("delim", C.c_char_p), ("wide_approx", C.c_int32)]
 
 
 class Desc(C.Structure):
@@ -48,7 +48,8 @@ class Regex(C.Structure):
 class Wide(C.Structure):
     _W = C.c_uint64 * WIDE_WORDS
     _fields_ = [("mask", _W * 256), ("init0", _W), ("init1", _W), ("noerr", _W), ("endpos", _W),
-                ("dendpos", _W), ("dmask", _W), ("reset", _W), ("start", _W)]
+                ("dendpos", _W), ("dmask", _W), ("reset", _W), ("start", _W),
+                ("reset_up", _W * AGB_MAXERR), ("start_up", _W * AGB_MAXERR)]
 
 
 class Record(C.Structure):

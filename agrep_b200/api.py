@@ -25,10 +25,13 @@ def _check_window(window):
 class Pattern:
     """agb_compile(): checksg() + preprocess() + maskgen() of the reference, plus the device plan.
     regex: accept regular expressions (a pattern with an unescaped '|' or '*': re() of the reference, k <= 4, lines);
-    without it such a pattern is refused."""
+    without it such a pattern is refused.
+    wide_approx: accept a simple literal of more than 63 positions (up to 255 characters) at k = 1..8, as the reference's
+    sgrep() does, in 320-bit rows; without it such a pattern is refused as too long."""
 
     def __init__(self, pattern, k=0, nocase=False, wordbound=False, wholeline=False, inverse=False,
-                 linenum=False, ins_free=False, cost_i=0, cost_s=0, cost_d=0, bestmatch=False, delim=None, regex=False):
+                 linenum=False, ins_free=False, cost_i=0, cost_s=0, cost_d=0, bestmatch=False, delim=None, regex=False,
+                 wide_approx=False):
         if isinstance(pattern, str):
             pattern = pattern.encode("latin-1")
         if isinstance(delim, str):
@@ -36,7 +39,8 @@ class Pattern:
         self.pattern = pattern
         self.opts = Options(k=k, nocase=int(nocase), wordbound=int(wordbound), wholeline=int(wholeline),
                             inverse=int(inverse), linenum=int(linenum), ins_free=int(ins_free),
-                            cost_i=cost_i, cost_s=cost_s, cost_d=cost_d, bestmatch=int(bestmatch), regex=int(regex), delim=delim)
+                            cost_i=cost_i, cost_s=cost_s, cost_d=cost_d, bestmatch=int(bestmatch), regex=int(regex), delim=delim,
+                            wide_approx=int(wide_approx))
         self._h = C.c_void_p()
         err = C.create_string_buffer(512)
         rc = _lib.lib().agb_compile(pattern, C.byref(self.opts), C.byref(self._h), err, 512)
@@ -56,8 +60,8 @@ class Pattern:
 
     @property
     def wide(self):
-        """the 320-bit words of a simple literal of more than 63 positions (a copy; word 0 = bits 0..63 of each row),
-        None for every other pattern"""
+        """the 320-bit words of a simple literal of more than 63 positions (a copy; word 0 = bits 0..63 of each row; row 0
+        of the post-delimiter and start rows in reset/start, rows 1..k in reset_up/start_up), None for every other pattern"""
         w = _lib.lib().agb_pattern_wide(self._h)
         return Wide.from_buffer_copy(w.contents) if w else None
 

@@ -23,7 +23,7 @@ template <> __device__ __forceinline__ uint32_t shift1<uint32_t>(uint32_t x)
 	return r;
 }
 
-/* a 320-bit row (agb_wide: a simple literal of more than 63 positions, k = 0), word 0 = bits 0..63.  The kernels only
+/* a 320-bit row (agb_wide: a simple literal of more than 63 positions, k = 0..8), word 0 = bits 0..63.  The kernels only
  * AND/OR/complement/compare rows and shift them right by one, so this is all a row needs. */
 struct Wide {
 	uint64_t w[AGB_WIDE_WORDS];
@@ -68,10 +68,10 @@ template <typename T, int NR>
 __device__ __forceinline__ void shared_init(RecShared<T, NR> &S, DevConsts<T> &C, const agb_desc *D, int nthreads, const void *wide = nullptr)
 {
 	if constexpr (std::is_same<T, Wide>::value) {
-		static_assert(NR == 1, "320-bit rows are k = 0 only");
 		const agb_wide *X = static_cast<const agb_wide *>(wide);
 		for (int i = threadIdx.x; i < 256; i += nthreads) S.mask[i] = Wide::load(X->mask[i]);
 		if (threadIdx.x == 0) { S.reset[0] = Wide::load(X->reset); S.start[0] = Wide::load(X->start); }
+		if (threadIdx.x >= 1 && threadIdx.x < NR) { S.reset[threadIdx.x] = Wide::load(X->reset_up[threadIdx.x - 1]); S.start[threadIdx.x] = Wide::load(X->start_up[threadIdx.x - 1]); }
 		C.init1 = Wide::load(X->init1); C.noerr = Wide::load(X->noerr); C.endpos = Wide::load(X->endpos); C.dendpos = Wide::load(X->dendpos);
 	} else {
 		for (int i = threadIdx.x; i < 256; i += nthreads) S.mask[i] = mirror<T>((T)D->mask[i]);

@@ -578,6 +578,7 @@ int sgrep(unsigned char *in_pat, int in_m, int fd, int D, int samepattern)
 	if (in_m < 1 || in_m >= (int)sizeof pat) { errno = AGREP_ERROR; return -1; }
 	memcpy(pat, in_pat, (size_t)in_m); pat[in_m] = 0;
 	o.k = D; o.wordbound = WORDBOUND; o.wholeline = WHOLELINE; o.inverse = (INVERSE && !COUNT) ? 1 : 0; o.nocase = NOUPPER;
+	o.wide_approx = 1;                                                         /* up to 255 characters at k > 0 too (sgrep.c:303) */
 	if (DELIMITER) {
 		/* D_pattern holds the delimiter bytes themselves here (agrep.c:3182-3185); re-escape for agb_compile */
 		int q = 0, t;

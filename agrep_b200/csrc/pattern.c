@@ -6,7 +6,8 @@
  * (maskgen.c:26-269: Mask[], Init[0], Init1, NO_ERR_MASK, endposition, D_endpos, wildmask) -- but is
  * organised as one pass over the user's pattern that emits automaton positions with 256-bit classes,
  * in 64-bit words (the reference stops at 32 positions, maskgen.c:201-208), or in the 320-bit words of agb_wide for a
- * simple literal of more than 63 positions at k = 0 (sgrep()'s bm()/monkey(), which take up to 255 characters).
+ * simple literal of more than 63 positions: at k = 0 (sgrep()'s bm()/monkey(), which take up to 255 characters), and at
+ * k = 1..8 when the caller asks for it (agb_options.wide_approx: the literals the reference hands to sgrep() at k > 0).
  *
  * It also derives what only the device path needs: the constant post-delimiter rows (asearch.c:175-186),
  * the delimiter kind, and the pigeonhole anchor plan for the front-end kernel.
@@ -37,7 +38,7 @@ typedef struct {
 typedef struct {
 	pos_t p[AGB_WIDE_MAXPOS + 4];
 	int n;               /* positions so far (1-based: p[1..n]) */
-	int wide_ok;         /* up to AGB_WIDE_MAXPOS positions (a simple literal at k = 0), else up to WIDTH - 1 */
+	int wide_ok;         /* up to AGB_WIDE_MAXPOS positions (a simple literal that sgrep() takes), else up to WIDTH - 1 */
 	int no_error, even;
 	int or_seen, and_mode, nparts;
 } build_t;
@@ -268,7 +269,7 @@ static void w_shr1(const uint64_t *x, uint64_t *r)
 	for (i = 0; i < AGB_WIDE_WORDS; i++) r[i] = (x[i] >> 1) | (i + 1 < AGB_WIDE_WORDS ? x[i + 1] << 63 : 0);
 }
 
-/* the words of finish() below in 320-bit rows, for a simple literal (SGREP_BM: no '#', no -p, no LUT, one separator).
+/* the words of finish() below in 320-bit rows, for a simple literal (no '#', no -p, no LUT, one separator).
  * The "everywhere but" masks fill the words up to the one that holds the feed bit M, so that M <= 63 gives the 64-bit
  * words in word 0 and zeros above */
 static int finish_wide(const build_t *b, agb_desc *d, agb_wide *w, char *err, size_t errlen)
@@ -348,7 +349,23 @@ static int delim_accepts(const agb_desc *d, const agb_wide *w, int c, int p)
 	return w ? w_has(w->mask[c], d->M - p) : (int)(d->mask[c] >> (d->M - p) & 1);
 }
 
-/* everything the device path needs beyond the reference's words; w: the words are those of agb_wide (k = 0) */
+/* reset_rows() and agbi_step() in 320-bit rows, unit costs (a simple literal is never AGB_ENGINE_ASEARCH1): one step from
+ * B[0..k] on the byte of mask cm; mask0: row 0 is masked with D_Mask before the upper rows read it */
+typedef uint64_t wrow_t[AGB_WIDE_WORDS];
+static void w_step(const agb_desc *d, const agb_wide *w, const wrow_t *B, wrow_t *A, const uint64_t *cm, int mask0)
+{
+	uint64_t s[AGB_WIDE_WORDS], t[AGB_WIDE_WORDS], u[AGB_WIDE_WORDS]; int r, i;
+	w_shr1(B[0], s);
+	for (i = 0; i < AGB_WIDE_WORDS; i++) A[0][i] = ((s[i] & cm[i]) | (w->init1[i] & B[0][i])) & (mask0 ? w->dmask[i] : ~0ull);
+	for (r = 1; r <= d->k; r++) {
+		w_shr1(B[r], s);
+		for (i = 0; i < AGB_WIDE_WORDS; i++) u[i] = A[r - 1][i] | B[r - 1][i];
+		w_shr1(u, t);
+		for (i = 0; i < AGB_WIDE_WORDS; i++) A[r][i] = (s[i] & cm[i]) | (w->init1[i] & B[r][i]) | B[r - 1][i] | (t[i] & w->noerr[i]);
+	}
+}
+
+/* everything the device path needs beyond the reference's words; w: the words are those of agb_wide */
 int agbi_derive(agb_desc *d, char *err, size_t errlen) { return derive(d, NULL, err, errlen); }
 
 static int derive(agb_desc *d, agb_wide *w, char *err, size_t errlen)
@@ -356,7 +373,7 @@ static int derive(agb_desc *d, agb_wide *w, char *err, size_t errlen)
 	int L = d->L, p, r;
 	uint64_t B[2 * AGB_MAXERR + 1], A[2 * AGB_MAXERR + 1];
 	if (L < 1 || L > AGB_MAXDELIM || d->M < L + 1 || d->M > (w ? AGB_WIDE_MAXPOS : WIDTH - 1)) FAIL("bad descriptor (M=%d, L=%d)", d->M, L);
-	if (d->k < 0 || d->k > AGB_MAXERR || (w && d->k)) FAIL("bad descriptor (k=%d)", d->k);
+	if (d->k < 0 || d->k > AGB_MAXERR) FAIL("bad descriptor (k=%d)", d->k);
 	if (w ? !w_has(w->dendpos, d->M - L) : !d->dendpos) FAIL("internal: delimiter end bit missing");
 	/* the device also recognises delimiters away from the automaton (record starts, ordinals), by their bytes: position p
 	 * of the delimiter must accept delim[p-1] and nothing else (-i with letters in the delimiter makes it accept both cases) */
@@ -383,13 +400,17 @@ static int derive(agb_desc *d, agb_wide *w, char *err, size_t errlen)
 	}
 	d->nrows = d->k + 1;
 	if (w) {
-		/* one row: reset_rows() and the virtual '\n' below, in 320 bits */
-		uint64_t s[AGB_WIDE_WORDS], a[AGB_WIDE_WORDS]; int i, hit = 0;
-		w_shr1(w->init0, s);
-		for (i = 0; i < AGB_WIDE_WORDS; i++) w->reset[i] = ((s[i] & w->mask[d->delim[L - 1]][i]) | (w->init1[i] & w->init0[i])) & w->dmask[i];
-		for (i = 0; i < AGB_WIDE_WORDS; i++) { a[i] = (s[i] & w->mask['\n'][i]) | (w->init1[i] & w->init0[i]); hit |= (a[i] & w->dendpos[i]) != 0; }
+		/* rows 0..k: reset_rows() and the virtual '\n' below, in 320 bits.  Row 0 goes to reset/start, rows 1..k to
+		 * reset_up/start_up */
+		wrow_t WB[AGB_MAXERR + 1], RA[AGB_MAXERR + 1], SA[AGB_MAXERR + 1]; int i, hit = 0;
+		for (r = 0; r <= d->k; r++) memcpy(WB[r], w->init0, sizeof WB[r]);
+		w_step(d, w, (const wrow_t *)WB, RA, w->mask[d->delim[L - 1]], 1);
+		w_step(d, w, (const wrow_t *)WB, SA, w->mask['\n'], 0);
+		for (i = 0; i < AGB_WIDE_WORDS; i++) hit |= (SA[0][i] & w->dendpos[i]) != 0;
 		d->start_closes = hit;
-		memcpy(w->start, hit ? w->reset : a, sizeof a);
+		if (hit) memcpy(SA, RA, sizeof SA);
+		memcpy(w->reset, RA[0], sizeof w->reset); memcpy(w->start, SA[0], sizeof w->start);
+		for (r = 1; r <= d->k; r++) { memcpy(w->reset_up[r - 1], RA[r], sizeof RA[r]); memcpy(w->start_up[r - 1], SA[r], sizeof SA[r]); }
 		return 0;
 	}
 	reset_rows(d, d->mask[d->delim[L - 1]], d->reset);
@@ -835,7 +856,7 @@ int agbi_build_rx(const char *pattern, const agb_options *o, agb_desc *d, agb_re
 		/* sgrep.c:289-320 + bm() :741-755: literal compared under TR[] (ASCII case folded, unconditional,
 		 * sgrep.c:226-236); -w = neither neighbour isalnum().  Stated as an exact automaton. */
 		int i;
-		b->wide_ok = wide != NULL;
+		b->wide_ok = wide != NULL;                                             /* (sgrep() takes up to 255 characters) */
 		if (o->wordbound) { pos_t *p = new_pos(b); int c; if (p) { p->prot = 1; for (c = 0; c < 256; c++) if (!is_alnum(c)) cls_set(p, c); } else rc = AGB_ERR_PATTERN; }
 		for (i = 0; i < m && !rc; i++) {
 			int c = s[i]; pos_t *p;
@@ -849,6 +870,8 @@ int agbi_build_rx(const char *pattern, const agb_options *o, agb_desc *d, agb_re
 		}
 		if (!rc && o->wordbound) { pos_t *p = new_pos(b); int c; if (p) { p->prot = 1; for (c = 0; c < 256; c++) if (!is_alnum(c)) cls_set(p, c); } else rc = AGB_ERR_PATTERN; }
 	} else if (!rc) {
+		/* a simple literal at k > 0, which the reference hands to sgrep() too: as many positions when the caller asks for it */
+		b->wide_ok = wide != NULL && sg && o->k > 0 && o->wide_approx;
 		if (o->wholeline) {                                                    /* preproce.c:148-159, maskgen.c:188-193 */
 			pos_t *p = new_pos(b); if (p) { p->prot = 1; cls_set(p, '\n'); cls_set(p, S_NNLINE); } else rc = AGB_ERR_PATTERN;
 		} else if (o->wordbound) rc = add_wordb(b, err, errlen);               /* preproce.c:161-166 */
@@ -859,7 +882,7 @@ int agbi_build_rx(const char *pattern, const agb_options *o, agb_desc *d, agb_re
 	if (rc) { if (err && errlen && !err[0]) snprintf(err, errlen, "pattern too long (has > %d chars)", WIDTH); free(b); return AGB_ERR_PATTERN; }
 	if (d->engine == AGB_ENGINE_BITAP && o->nocase) { agbi_lut_lower1(lut); rc = finish(b, d, o, lut, err, errlen); }
 	else if (b->wide_ok && (b->n > WIDTH - 1 || (getenv("AGB_FORCE_WIDE") && atoi(getenv("AGB_FORCE_WIDE")) == 1)))
-		rc = finish_wide(b, d, wide, err, errlen);                             /* (AGB_FORCE_WIDE=1: every simple literal, for tests) */
+		rc = finish_wide(b, d, wide, err, errlen);                             /* (AGB_FORCE_WIDE=1: every such literal, for tests) */
 	else rc = finish(b, d, o, NULL, err, errlen);
 	if (!rc) plan_anchors(b, d, o, d->engine == AGB_ENGINE_SGREP_BM);
 	free(b);

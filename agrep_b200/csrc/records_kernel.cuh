@@ -319,8 +319,10 @@ k_records_dense(const RecParams P0)
 #define LIST_NG (LIST_GB + 1 + LIST_GA)
 #define LIST_STRIDE (LIST_NG * 4 + 1)                   /* words; odd: the lanes of a warp hit different banks */
 #define LIST_SMEM (REC_THREADS * LIST_STRIDE * 4)
+/* 320-bit rows: 2 blocks per SM, so that the rows of k = 1..8 stay in registers (at 6 they go to local memory) */
+template <typename T> constexpr int list_min_blocks() { return std::is_same<T, Wide>::value ? 2 : 6; }
 template <typename T, int NR, bool COSTS>
-__global__ void __launch_bounds__(REC_THREADS, 6)
+__global__ void __launch_bounds__(REC_THREADS, list_min_blocks<T>())
 k_records_list(const RecParams P)
 {
 	extern __shared__ __align__(16) uint32_t s_win[];
@@ -384,6 +386,45 @@ static void launch_dense_one(const RecParams &P, unsigned grid, cudaStream_t st)
 		configured[dev & 63] = true;
 	}
 	k_records_dense<T, NR, COSTS, SET><<<grid, DENSE_THREADS, DENSE_SMEM, st>>>(P);
+}
+
+/* the launchers at a row count known at run time (1..9; -1 for any other) */
+template <typename T, bool COSTS, bool SET>
+static int launch_dense_t(int nrows, const RecParams &P, unsigned grid, cudaStream_t st)
+{
+	switch (nrows) {
+	case 1: launch_dense_one<T, 1, COSTS, SET>(P, grid, st); break;
+	case 2: launch_dense_one<T, 2, COSTS, SET>(P, grid, st); break;
+	case 3: launch_dense_one<T, 3, COSTS, SET>(P, grid, st); break;
+	case 4: launch_dense_one<T, 4, COSTS, SET>(P, grid, st); break;
+	case 5: launch_dense_one<T, 5, COSTS, SET>(P, grid, st); break;
+	case 6: launch_dense_one<T, 6, COSTS, SET>(P, grid, st); break;
+	case 7: launch_dense_one<T, 7, COSTS, SET>(P, grid, st); break;
+	case 8: launch_dense_one<T, 8, COSTS, SET>(P, grid, st); break;
+	case 9: launch_dense_one<T, 9, COSTS, SET>(P, grid, st); break;
+	default: return -1;
+	}
+	g_launches++;
+	return 0;
+}
+
+template <typename T, bool COSTS>
+static int launch_records_list_t(int nrows, const RecParams &P, unsigned grid, cudaStream_t st)
+{
+	switch (nrows) {
+	case 1: k_records_list<T, 1, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
+	case 2: k_records_list<T, 2, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
+	case 3: k_records_list<T, 3, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
+	case 4: k_records_list<T, 4, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
+	case 5: k_records_list<T, 5, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
+	case 6: k_records_list<T, 6, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
+	case 7: k_records_list<T, 7, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
+	case 8: k_records_list<T, 8, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
+	case 9: k_records_list<T, 9, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
+	default: return -1;
+	}
+	g_launches++;
+	return 0;
 }
 
 #endif

@@ -221,8 +221,8 @@ int  launch_regex_set(const agb_desc &d, const RecParams &P, unsigned grid, cuda
 int  launch_records_list(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 /* records_wide.cu: the same forms for 320-bit rows (agb_desc.wide: the words in RecParams.rx_tab), which the launchers
  * above hand over to */
-int  launch_dense_wide(const RecParams &P, unsigned grid, cudaStream_t st, bool set);
-int  launch_records_list_wide(const RecParams &P, unsigned grid, cudaStream_t st);
+int  launch_dense_wide(int nrows, const RecParams &P, unsigned grid, cudaStream_t st, bool set);
+int  launch_records_list_wide(int nrows, const RecParams &P, unsigned grid, cudaStream_t st);
 int  launch_slices(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 bool slices_usable(const agb_desc &d);
 /* regex.cu: stage 2 of AGB_ENGINE_REGEX (RecParams.rx_tab set), and its tables (returns the bytes written: 32- or 64-bit words) */

@@ -50,6 +50,8 @@ typedef struct agb_options {
 	int32_t regex;        /* 1: accept regular expressions (an unescaped '|' or '*', preproce.c:139-142) as
 	                         AGB_ENGINE_REGEX; 0: refuse them                                 */
 	const char *delim;    /* -d  argument as typed, NULL = newline records                   */
+	int32_t wide_approx;  /* 1: accept a simple literal of 64 to AGB_WIDE_MAXPOS positions at k = 1..8 (what the
+	                         reference's sgrep() takes, up to 255 characters) in 320-bit rows; 0: refuse it     */
 } agb_options;
 
 /* engines = which reference function the descriptor stands for */
@@ -124,20 +126,23 @@ typedef struct agb_regex {
 	int32_t  pad[2];
 } agb_regex;
 
-/* What a simple literal of more than 63 positions adds to the descriptor (AGB_ENGINE_SGREP_BM, k = 0: sgrep()'s bm() and
- * monkey(), up to 255 characters as the reference accepts them, agrep.c:3057): the words of 320-bit rows.  Word 0 holds bits
+/* What a simple literal of more than 63 positions adds to the descriptor (sgrep()'s bm() and monkey() at k = 0, up to 255
+ * characters as the reference accepts them, agrep.c:3057; at k = 1..8 with agb_options.wide_approx, the automaton the
+ * engines AGB_ENGINE_ASEARCH/ASEARCH0 run for shorter simple literals): the words of 320-bit rows.  Word 0 holds bits
  * 0..63 of a row; position p is bit M-p, the always-on feed is bit M, as in the descriptor.  Masks that the descriptor
  * fills "everywhere but" (init0's feed, noerr, dmask) are filled up to the end of the last word that holds bit M, and the
  * words above it are zero, so a pattern of at most 63 positions has exactly its 64-bit words in word 0.  The descriptor of
- * such a pattern has wide = 1, k = 0, nrows = 1, its real M and everything that is not a word (L, delim, delim_fold,
+ * such a pattern has wide = 1, its k, nrows = k + 1, its real M and everything that is not a word (L, delim, delim_fold,
  * delim_kind, engine, plan, anchors, pat_len, start_closes, inverse, user_delim, outtail); its 64-bit word fields (mask,
- * init0 ... wildmask, reset, start) are zero. */
+ * init0 ... wildmask, reset, start) are zero.  Row 0 of the post-delimiter and start rows is in reset/start, rows 1..k in
+ * reset_up[0..k-1]/start_up[0..k-1] (appended, so that the layout of the k = 0 fields stays put). */
 #define AGB_WIDE_WORDS  5
 #define AGB_WIDE_MAXPOS (64 * AGB_WIDE_WORDS - 1)
 typedef struct agb_wide {
 	uint64_t mask[256][AGB_WIDE_WORDS];
 	uint64_t init0[AGB_WIDE_WORDS], init1[AGB_WIDE_WORDS], noerr[AGB_WIDE_WORDS], endpos[AGB_WIDE_WORDS];
 	uint64_t dendpos[AGB_WIDE_WORDS], dmask[AGB_WIDE_WORDS], reset[AGB_WIDE_WORDS], start[AGB_WIDE_WORDS];
+	uint64_t reset_up[AGB_MAXERR][AGB_WIDE_WORDS], start_up[AGB_MAXERR][AGB_WIDE_WORDS];
 } agb_wide;
 
 /* one matching record, in the reference's own terms (file offsets, not buffer indexes):
@@ -185,7 +190,8 @@ const agb_regex *agb_pattern_regex(const agb_pattern *p);
 int  agb_pattern_from_regex(const agb_desc *d, const agb_regex *rx, agb_pattern **out, char *err, size_t errlen);
 /* the 320-bit words of a simple literal of more than 63 positions (NULL for every other pattern).  agb_pattern_from_desc
  * refuses such descriptors: the drop-in's sgrep() compiles from the pattern text.  With AGB_FORCE_WIDE=1 in the
- * environment agb_compile gives every AGB_ENGINE_SGREP_BM pattern this form (tests compare the two forms with it). */
+ * environment agb_compile gives every AGB_ENGINE_SGREP_BM pattern this form, and with agb_options.wide_approx every simple
+ * literal at k >= 1 (tests compare the two forms with it). */
 const agb_wide *agb_pattern_wide(const agb_pattern *p);
 
 /* ---- device scan ----
