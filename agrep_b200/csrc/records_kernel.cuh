@@ -392,39 +392,13 @@ static void launch_dense_one(const RecParams &P, unsigned grid, cudaStream_t st)
 template <typename T, bool COSTS, bool SET>
 static int launch_dense_t(int nrows, const RecParams &P, unsigned grid, cudaStream_t st)
 {
-	switch (nrows) {
-	case 1: launch_dense_one<T, 1, COSTS, SET>(P, grid, st); break;
-	case 2: launch_dense_one<T, 2, COSTS, SET>(P, grid, st); break;
-	case 3: launch_dense_one<T, 3, COSTS, SET>(P, grid, st); break;
-	case 4: launch_dense_one<T, 4, COSTS, SET>(P, grid, st); break;
-	case 5: launch_dense_one<T, 5, COSTS, SET>(P, grid, st); break;
-	case 6: launch_dense_one<T, 6, COSTS, SET>(P, grid, st); break;
-	case 7: launch_dense_one<T, 7, COSTS, SET>(P, grid, st); break;
-	case 8: launch_dense_one<T, 8, COSTS, SET>(P, grid, st); break;
-	case 9: launch_dense_one<T, 9, COSTS, SET>(P, grid, st); break;
-	default: return -1;
-	}
-	g_launches++;
-	return 0;
+	return launch_rows<9>(nrows, [&](auto R) { launch_dense_one<T, decltype(R)::value, COSTS, SET>(P, grid, st); });
 }
 
 template <typename T, bool COSTS>
 static int launch_records_list_t(int nrows, const RecParams &P, unsigned grid, cudaStream_t st)
 {
-	switch (nrows) {
-	case 1: k_records_list<T, 1, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
-	case 2: k_records_list<T, 2, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
-	case 3: k_records_list<T, 3, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
-	case 4: k_records_list<T, 4, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
-	case 5: k_records_list<T, 5, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
-	case 6: k_records_list<T, 6, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
-	case 7: k_records_list<T, 7, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
-	case 8: k_records_list<T, 8, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
-	case 9: k_records_list<T, 9, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); break;
-	default: return -1;
-	}
-	g_launches++;
-	return 0;
+	return launch_rows<9>(nrows, [&](auto R) { k_records_list<T, decltype(R)::value, COSTS><<<grid, REC_THREADS, LIST_SMEM, st>>>(P); });
 }
 
 #endif

@@ -226,16 +226,7 @@ static void launch_regex_one(const RecParams &P, unsigned grid, cudaStream_t st)
 template <typename T, bool LEVELS, bool SET>
 static int launch_regex_t(int nrows, const RecParams &P, unsigned grid, cudaStream_t st)
 {
-	switch (nrows) {
-	case 1: launch_regex_one<T, 1, LEVELS, SET>(P, grid, st); break;
-	case 2: launch_regex_one<T, 2, LEVELS, SET>(P, grid, st); break;
-	case 3: launch_regex_one<T, 3, LEVELS, SET>(P, grid, st); break;
-	case 4: launch_regex_one<T, 4, LEVELS, SET>(P, grid, st); break;
-	case 5: launch_regex_one<T, 5, LEVELS, SET>(P, grid, st); break;
-	default: return -1;
-	}
-	g_launches++;
-	return 0;
+	return launch_rows<5>(nrows, [&](auto R) { launch_regex_one<T, decltype(R)::value, LEVELS, SET>(P, grid, st); });
 }
 
 /* 32-bit words hold positions 0..31 (M <= 31), 64-bit words the rest */

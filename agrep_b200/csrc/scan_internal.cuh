@@ -19,6 +19,7 @@
 #include <stdlib.h>
 #include <atomic>
 #include <algorithm>
+#include <type_traits>
 
 extern thread_local char g_err[512];
 extern std::atomic<uint64_t> g_launches;
@@ -157,6 +158,16 @@ __device__ __forceinline__ bool rec_owned(const RecParams &P, int64_t begin, int
 	if (oe < P.own_lo || oe >= P.own_hi) return false;
 	if (!P.shard_last && close_pos >= (int64_t)P.n) P.totals[11] = 1ull;
 	return true;
+}
+
+/* a record-stage launcher at a row count known at run time: launch(std::integral_constant<int, nrows>()) for
+ * 1 <= nrows <= N, counted in g_launches; -1 for any other row count */
+template <int N, typename F>
+static int launch_rows(int nrows, const F &launch)
+{
+	if (nrows == N) { launch(std::integral_constant<int, N>()); g_launches++; return 0; }
+	if constexpr (N > 1) return launch_rows<N - 1>(nrows, launch);
+	return -1;
 }
 
 /* ---- host ---- */

@@ -299,20 +299,7 @@ static void launch_slices_one(const RecParams &P, unsigned grid, cudaStream_t st
 template <typename T, bool COSTS>
 static int launch_slices_t(int nrows, const RecParams &P, unsigned grid, cudaStream_t st)
 {
-	switch (nrows) {
-	case 1: launch_slices_one<T, 1, COSTS>(P, grid, st); break;
-	case 2: launch_slices_one<T, 2, COSTS>(P, grid, st); break;
-	case 3: launch_slices_one<T, 3, COSTS>(P, grid, st); break;
-	case 4: launch_slices_one<T, 4, COSTS>(P, grid, st); break;
-	case 5: launch_slices_one<T, 5, COSTS>(P, grid, st); break;
-	case 6: launch_slices_one<T, 6, COSTS>(P, grid, st); break;
-	case 7: launch_slices_one<T, 7, COSTS>(P, grid, st); break;
-	case 8: launch_slices_one<T, 8, COSTS>(P, grid, st); break;
-	case 9: launch_slices_one<T, 9, COSTS>(P, grid, st); break;
-	default: return -1;
-	}
-	g_launches++;
-	return 0;
+	return launch_rows<9>(nrows, [&](auto R) { launch_slices_one<T, decltype(R)::value, COSTS>(P, grid, st); });
 }
 int launch_slices(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st)
 {
