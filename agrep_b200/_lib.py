@@ -20,7 +20,8 @@ class Options(C.Structure):
     _fields_ = [("k", C.c_int32), ("nocase", C.c_int32), ("wordbound", C.c_int32), ("wholeline", C.c_int32),
                 ("inverse", C.c_int32), ("linenum", C.c_int32), ("ins_free", C.c_int32),
                 ("cost_i", C.c_int32), ("cost_s", C.c_int32), ("cost_d", C.c_int32),
-                ("bestmatch", C.c_int32), ("regex", C.c_int32), ("delim", C.c_char_p), ("wide_approx", C.c_int32)]
+                ("bestmatch", C.c_int32), ("regex", C.c_int32), ("delim", C.c_char_p), ("wide_approx", C.c_int32),
+                ("sticky_delim", C.c_int32)]
 
 
 class Desc(C.Structure):
@@ -38,7 +39,8 @@ class Desc(C.Structure):
                 ("anchor", C.c_uint32 * AGB_MAXANCHOR), ("anchor_fold", C.c_uint32), ("anchor_mask", C.c_uint32),
                 ("refine", C.c_int32), ("pat_len", C.c_int32), ("anchor_off", C.c_int32 * AGB_MAXANCHOR),
                 ("n_anchors3", C.c_int32), ("anchor3", C.c_uint32 * 4), ("anchor3_off", C.c_int32 * 4), ("adaptive", C.c_int32),
-                ("delim_fold", C.c_uint8 * (2 * AGB_MAXDELIM + 2)), ("pair_plan", C.c_uint8), ("wide", C.c_uint8)]
+                ("delim_fold", C.c_uint8 * (2 * AGB_MAXDELIM + 2)), ("pair_plan", C.c_uint8), ("wide", C.c_uint8),
+                ("sticky_delim", C.c_uint8)]
 
 
 class Regex(C.Structure):

@@ -27,11 +27,14 @@ class Pattern:
     regex: accept regular expressions (a pattern with an unescaped '|' or '*': re() of the reference, k <= 4, lines);
     without it such a pattern is refused.
     wide_approx: accept a simple literal of more than 63 positions (up to 255 characters) at k = 1..8, as the reference's
-    sgrep() does, in 320-bit rows; without it such a pattern is refused as too long."""
+    sgrep() does, in 320-bit rows; without it such a pattern is refused as too long.
+    sticky_delim: accept ins_free (-p) with a delimiter of two or more bytes, as the reference does: its positions are
+    sticky too, so a record closes where the delimiter's bytes have occurred in order since the last close ("a ... b"
+    for "ab"); without it such a pattern is refused.  The sharded scans refuse it either way."""
 
     def __init__(self, pattern, k=0, nocase=False, wordbound=False, wholeline=False, inverse=False,
                  linenum=False, ins_free=False, cost_i=0, cost_s=0, cost_d=0, bestmatch=False, delim=None, regex=False,
-                 wide_approx=False):
+                 wide_approx=False, sticky_delim=False):
         if isinstance(pattern, str):
             pattern = pattern.encode("latin-1")
         if isinstance(delim, str):
@@ -40,7 +43,7 @@ class Pattern:
         self.opts = Options(k=k, nocase=int(nocase), wordbound=int(wordbound), wholeline=int(wholeline),
                             inverse=int(inverse), linenum=int(linenum), ins_free=int(ins_free),
                             cost_i=cost_i, cost_s=cost_s, cost_d=cost_d, bestmatch=int(bestmatch), regex=int(regex), delim=delim,
-                            wide_approx=int(wide_approx))
+                            wide_approx=int(wide_approx), sticky_delim=int(sticky_delim))
         self._h = C.c_void_p()
         err = C.create_string_buffer(512)
         rc = _lib.lib().agb_compile(pattern, C.byref(self.opts), C.byref(self._h), err, 512)

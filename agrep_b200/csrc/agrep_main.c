@@ -239,6 +239,7 @@ int main(int argc, char **argv)
 	memset(&o, 0, sizeof o);
 	o.regex = 1;
 	o.wide_approx = 1;                       /* long simple literals at k > 0, as the reference's sgrep() takes them */
+	o.sticky_delim = 1;                      /* -p with a delimiter of two or more bytes, as the reference answers it */
 	if (argc > 0 && argv[0]) { const char *s = strrchr(argv[0], '/'); prog = s ? s + 1 : argv[0]; }
 	for (ai = 1; ai < argc && argv[ai][0] == '-' && argv[ai][1]; ai++) {
 		const char *q = argv[ai] + 1; int stop = 0;

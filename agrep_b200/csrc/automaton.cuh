@@ -164,6 +164,16 @@ __device__ __forceinline__ bool delim_ends_at(RD &R, int64_t q, const uint8_t *d
 	return (len % L) == 0;
 }
 
+/* delim_kind 3 (-p, L >= 2): the delimiter's state s (positions 1..s taken since the last close) on byte c, which takes
+ * position s + 1 or not; the L-th closes the record and starts over (delim_state.cu).  true: c closes a record */
+__device__ __forceinline__ bool dstate_step(int &s, int c, const uint8_t *delim, const uint8_t *dfold, int L)
+{
+	if ((c | dfold[s]) != delim[s]) return false;
+	if (++s < L) return false;
+	s = 0;
+	return true;
+}
+
 /* one text byte through all rows: asearch.c:96-115 (unit costs), asearch1.c:88-97 (COSTS), bitap.c:175-176 (NR = 1) */
 template <typename T, int NR, bool COSTS>
 __device__ __forceinline__ void rows_step(T (&S)[NR], T cm, const DevConsts<T> &C)

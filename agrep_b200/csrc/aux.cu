@@ -273,9 +273,13 @@ extern "C" int agb_corpus_fill_host(const agb_corpus_spec *s, void *h_text)
 
 /* delimiter ends in [from, to) (file offsets; to <= n + L), sequentially; run: the length of the run of delim[0]
  * that ends at from - 1 (kind 1) */
-__device__ __forceinline__ uint32_t ord_count_seq(Reader &R, const OrdParams &P, int64_t from, int64_t to)
+__device__ __forceinline__ uint32_t ord_count_seq(Reader &R, const OrdParams &P, int64_t from, int64_t to, int ds = 0)
 {
 	uint32_t cnt = 0;
+	if (P.kind == 3) {                           /* ds: the delimiter's state at from (delim_state.cu) */
+		for (int64_t q = from; q < to; q++) cnt += dstate_step(ds, R.get(q), P.delim, P.dfold, P.L) ? 1u : 0u;
+		return cnt;
+	}
 	if (P.L == 1) { for (int64_t q = from; q < to; q++) cnt += (R.get(q) | P.dfold[0]) == P.delim[0]; return cnt; }
 	if (P.kind == 0) {
 		for (int64_t q = from; q < to; q++) {
@@ -338,7 +342,8 @@ k_delim_count(const OrdParams P0, const SetFile *set_files = nullptr, const SetT
 		const int64_t s0 = tile0 + (int64_t)tid * ORD_PER, s1 = s0 + ORD_PER < limit ? s0 + ORD_PER : limit;
 		if (s0 < limit) {
 			Reader R; R.init(P.text, P.n, P.delim, P.L);
-			cnt = ord_count_seq(R, P, s0, s1);
+			const uint64_t gtile = SET ? (uint64_t)set_files[file].ord_tile0 + tile_ : blockIdx.x;
+			cnt = ord_count_seq(R, P, s0, s1, P.kind == 3 ? P.dstate[gtile * ORD_THREADS + tid] : 0);
 		}
 		uint32_t b = cnt;
 		b += __shfl_xor_sync(0xffffffffu, b, 1); b += __shfl_xor_sync(0xffffffffu, b, 2);
@@ -408,7 +413,7 @@ __global__ void __launch_bounds__(256) k_ordinals(const OrdParams P)
 	unsigned long long j = P.tile_off[tile];
 	for (uint64_t b = tile * (ORD_TILE / ORD_BLOCK); b < blk; b++) j += P.blocks[b];
 	if (P.L == 1) j += ord_count_swar(P, (int64_t)(blk * ORD_BLOCK), q + 1);
-	else { Reader R; R.init(P.text, P.n, P.delim, P.L); j += ord_count_seq(R, P, (int64_t)(blk * ORD_BLOCK), q + 1); }
+	else { Reader R; R.init(P.text, P.n, P.delim, P.L); j += ord_count_seq(R, P, (int64_t)(blk * ORD_BLOCK), q + 1, P.kind == 3 ? P.dstate[blk * (ORD_BLOCK / ORD_PER)] : 0); }
 	/* the virtual '\n' closes a record of its own when it completes a delimiter: only a 1-byte '\n' can */
 	const long long virt = (P.L == 1 && P.delim[0] == '\n') ? 1 : 0;
 	P.records[i].ordinal = (long long)j + virt + P.j0;
@@ -430,7 +435,10 @@ __global__ void __launch_bounds__(256) k_ordinals_set(const OrdParams P0, const 
 	unsigned long long j = P.tile_off[tile] - P.tile_off[f.ord_tile0];
 	for (uint64_t b = b0; b < b0 + (uint64_t)(q % ORD_TILE) / ORD_BLOCK; b++) j += P.blocks[b];
 	if (P.L == 1) j += ord_count_swar(P, (int64_t)(blk * ORD_BLOCK), q + 1);
-	else { Reader R; R.init(P.text, P.n, P.delim, P.L); j += ord_count_seq(R, P, (int64_t)(blk * ORD_BLOCK), q + 1); }
+	else {
+		Reader R; R.init(P.text, P.n, P.delim, P.L);
+		j += ord_count_seq(R, P, (int64_t)(blk * ORD_BLOCK), q + 1, P.kind == 3 ? P.dstate[tile * ORD_THREADS + (uint64_t)(q % ORD_TILE) / ORD_BLOCK * (ORD_BLOCK / ORD_PER)] : 0);
+	}
 	const long long virt = (P.L == 1 && P.delim[0] == '\n') ? 1 : 0;
 	P.records[i].ordinal = (long long)j + virt + f.j0;
 }
@@ -483,7 +491,7 @@ int ordinals_launch(const agb_desc &d, Workspace &W, const void *d_text, uint64_
 	P.text = (const uint8_t *)d_text; P.n = n; P.blocks = W.ord_blocks; P.tiles = W.tile_counts; P.tile_off = W.tile_offsets;
 	P.records = d_records; P.totals = W.totals; P.capacity = capacity;
 	for (int i = 0; i < AGB_MAXDELIM + 2; i++) { P.dfold[i] = d.delim_fold[i]; P.delim[i] = d.delim[i] | d.delim_fold[i]; }
-	P.L = d.L; P.kind = d.delim_kind;
+	P.L = d.L; P.kind = d.delim_kind; P.dstate = W.dstate;
 	W.ord_virt = (d.L == 1 && d.delim[0] == '\n') ? 1 : 0;
 	/* bitap.c:151-156: j starts at -1 when the text begins with the user's delimiter (asearch0() has no such correction) */
 	/* (this one check is byte for byte against the delimiter as typed, also under -i: bitap.c:151-154 compares old_D_pat) */
@@ -527,7 +535,7 @@ int ordinals_set_launch(const agb_desc &d, Workspace &W, const void *d_text, con
 	P.text = (const uint8_t *)d_text; P.blocks = W.ord_blocks; P.tiles = W.tile_counts; P.tile_off = W.tile_offsets;
 	P.records = d_records; P.totals = W.totals; P.capacity = capacity;
 	for (int i = 0; i < AGB_MAXDELIM + 2; i++) { P.dfold[i] = d.delim_fold[i]; P.delim[i] = d.delim[i] | d.delim_fold[i]; }
-	P.L = d.L; P.kind = d.delim_kind;
+	P.L = d.L; P.kind = d.delim_kind; P.dstate = W.dstate;
 	k_delim_count<true><<<(unsigned)ord_tiles, ORD_THREADS, 0, st>>>(P, d_files, d_ord_tiles, d_stats); g_launches++;
 	k_scan_tiles<<<1, 1024, 0, st>>>(W.tile_counts, W.tile_offsets, ord_tiles, nullptr); g_launches++;
 	if (d_records && capacity) { k_ordinals_set<<<(unsigned)((capacity + 255) / 256), 256, 0, st>>>(P, d_files); g_launches++; }

@@ -273,6 +273,7 @@ static int desc_from_globals(agb_desc *d, const unsigned char *dpat, int L, cons
 	d->cost_i = I > D ? D + 1 : I; d->cost_s = S > D ? D + 1 : S; d->cost_d = DD > D ? D + 1 : DD;   /* asearch1.c:42-44 */
 	if (d->cost_i < 1) d->cost_i = 1;
 	if (Pattern) plan_from_internal(Pattern, L, D, d);
+	d->sticky_delim = 1;                                                      /* -p (I = 0) with a delimiter of two or more bytes */
 	return 0;
 }
 

@@ -379,8 +379,9 @@ static int derive(agb_desc *d, agb_wide *w, char *err, size_t errlen)
 	 * of the delimiter must accept delim[p-1] and nothing else (-i with letters in the delimiter makes it accept both cases) */
 	/* -p (Init1 all ones, bitap.c:123) makes every position sticky, the delimiter's too: with a delimiter of two or more
 	 * bytes "a ... b" then closes a record like "ab" does.  One byte is fine (its only position is D_endpos itself). */
-	if (d->init1 == ~0ull && L > 1)
+	if (d->init1 == ~0ull && L > 1 && !d->sticky_delim)
 		FAIL("-p with a delimiter of more than one byte is not supported (insertions inside the delimiter would be free too)");
+	if (d->init1 != ~0ull || L == 1) d->sticky_delim = 0;
 	memset(d->delim_fold, 0, sizeof d->delim_fold);
 	for (p = 1; p <= L; p++) {
 		int c, cnt = 0, lo = d->delim[p - 1] | 0x20;
@@ -393,7 +394,13 @@ static int derive(agb_desc *d, agb_wide *w, char *err, size_t errlen)
 	/* delimiter recognition away from the automaton (record-start search on the device) */
 	unsigned char fd[2 * AGB_MAXDELIM + 2];
 	folded_delim(d, fd);
-	if (L == 1 || !has_border(fd, L)) d->delim_kind = 0;
+	if (d->sticky_delim) {
+		/* the delimiter's state is a function of the text alone (its positions are fed by the always-on bits only): the device
+		 * scans it (delim_state.cu).  Free insertions leave no piece that a match must hold verbatim: no anchors */
+		d->delim_kind = 3;
+		d->plan = AGB_PLAN_ALL; d->n_anchors = 0; d->n_anchors3 = 0; d->refine = 0;
+	}
+	else if (L == 1 || !has_border(fd, L)) d->delim_kind = 0;
 	else {
 		for (p = 1; p < L; p++) if (fd[p] != fd[0]) break;
 		d->delim_kind = p < L ? 2 : 1;          /* a run such as $$, or any other self-overlap ("aba"): automaton.cuh delim_ends_at */
@@ -880,6 +887,7 @@ int agbi_build_rx(const char *pattern, const agb_options *o, agb_desc *d, agb_re
 		else if (!rc && o->wordbound) rc = add_wordb(b, err, errlen);          /* preproce.c:169-173 */
 	}
 	if (rc) { if (err && errlen && !err[0]) snprintf(err, errlen, "pattern too long (has > %d chars)", WIDTH); free(b); return AGB_ERR_PATTERN; }
+	d->sticky_delim = o->sticky_delim ? 1 : 0;                                  /* (derive() keeps it only where -p meets L >= 2) */
 	if (d->engine == AGB_ENGINE_BITAP && o->nocase) { agbi_lut_lower1(lut); rc = finish(b, d, o, lut, err, errlen); }
 	else if (b->wide_ok && (b->n > WIDTH - 1 || (getenv("AGB_FORCE_WIDE") && atoi(getenv("AGB_FORCE_WIDE")) == 1)))
 		rc = finish_wide(b, d, wide, err, errlen);                             /* (AGB_FORCE_WIDE=1: every such literal, for tests) */
@@ -952,7 +960,8 @@ const agb_desc *agb_pattern_desc(const agb_pattern *p) { return p ? &p->d : NULL
 
 /* j of the reference's loops (bitap.c:178, asearch.c:120): incremented at every record close, the virtual '\n'
  * included; pre-decremented when the text starts with the user's delimiter (bitap.c:151-156; asearch0() has no
- * such correction, asearch.c:609-612).  Same greedy delimiter rule as the device (scan.cu delim_ends_at). */
+ * such correction, asearch.c:609-612).  Same greedy delimiter rule as the device (scan.cu delim_ends_at), and for
+ * delim_kind 3 the delimiter's state machine of delim_state.cu. */
 void agb_fill_ordinals(const agb_pattern *p, const void *h_text, uint64_t n, agb_record *records, uint64_t n_records)
 {
 	const agb_desc *d = &p->d; const unsigned char *t = (const unsigned char *)h_text;
@@ -966,7 +975,11 @@ void agb_fill_ordinals(const agb_pattern *p, const void *h_text, uint64_t n, agb
 	/* position q = -1 is the virtual '\n'; positions n .. n+L-1 are the delimiter appended at EOF */
 	for (q = -1; q < (long long)n + L && i < n_records; q++) {
 		int c = q < 0 ? '\n' : (q < (long long)n ? t[q] : d->delim[q - (long long)n]), e;
-		if (L == 1) e = DEQ(c, 0);
+		if (d->delim_kind == 3) {
+			/* -p: position run + 1 of the delimiter takes c or not; the L-th closes and starts over (DESIGN 3.3.1) */
+			if (DEQ(c, run) && ++run == L) run = 0, e = 1; else e = 0;
+		}
+		else if (L == 1) e = DEQ(c, 0);
 		else if (d->delim_kind == 1) { run = DEQ(c, 0) ? run + 1 : 0; e = run > 0 && run % L == 0; }
 		else if (d->delim_kind == 2) {
 			/* occurrences are taken from the left; one that shares a byte with the one taken before it is dropped */

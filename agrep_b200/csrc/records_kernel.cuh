@@ -84,6 +84,26 @@ __device__ __forceinline__ uint32_t chunk_records(const RecParams &P, const DevC
 	return cnt;
 }
 
+/* delim_kind 3: the closes in a slice of DENSE_PER staged bytes (len of them in the text), walked from the delimiter's state
+ * at its start (bit j: at byte j).  Not inlined: the other delimiters' dense kernels keep their registers */
+static_assert(DENSE_PER == 128, "two words of close bits per slice");
+static __device__ __noinline__ ulonglong2 dstate_slice_closes(const uint8_t *sl, int64_t len, int ds, const uint8_t *delim, const uint8_t *dfold, int L)
+{
+	ulonglong2 w = make_ulonglong2(0, 0);
+	for (uint32_t v = 0; v < DENSE_PER / 16 && (int64_t)(16 * v) < len; v++) {
+		const uint4 x = *reinterpret_cast<const uint4 *>(sl + v * 16);
+		const uint32_t xs[4] = { x.x, x.y, x.z, x.w };
+#pragma unroll
+		for (uint32_t b = 0; b < 16; b++) {
+			const uint32_t j = 16 * v + b;
+			if ((int64_t)j < len && dstate_step(ds, (int)((xs[b >> 2] >> (8 * (b & 3))) & 0xFFu), delim, dfold, L)) {
+				if (j < 64) w.x |= 1ull << j; else w.y |= 1ull << (j - 64);
+			}
+		}
+	}
+	return w;
+}
+
 /* dense tile form: the automaton over EVERYTHING (no anchor plan: classes, -v, -p, '#', short patterns ...).
  * One CTA per 32 KiB tile, brought into shared memory (+2 KiB that follow it) by one bulk-async copy.  Thread t
  * owns the records whose opening delimiter ends inside its 128-byte slice: it starts at the first of them in the
@@ -145,6 +165,11 @@ k_records_dense(const RecParams P0)
 			}
 			bits[v >> 2] |= (uint64_t)m16 << (16 * (v & 3));
 		}
+	} else if (C.kind == 3) {
+		/* -p: one walk over the slice from the state the delimiter pass found at its start */
+		const uint64_t slice = SET ? ((uint64_t)P0.set_files[file].ord_tile0 + tile) * DENSE_THREADS + tid : (uint64_t)tile0 / DENSE_PER + tid;
+		const ulonglong2 w = dstate_slice_closes(s_text + tid * DENSE_PER, n - (tile0 + (int64_t)tid * DENSE_PER), P.dstate[slice], SH.delim, SH.dfold, L);
+		bits[0] = w.x; bits[1] = w.y;
 	} else {
 		for (uint32_t j = 0; j < DENSE_PER; j++) {
 			const int64_t q = tile0 + (int64_t)tid * DENSE_PER + j;
@@ -159,8 +184,9 @@ k_records_dense(const RecParams P0)
 			if (hi < 0) bits[w] = 0; else if (hi < 63) bits[w] &= (2ull << hi) - 1;
 		}
 	}
-	/* the very first record of the text has no delimiter in front of it: thread 0 of tile 0 */
-	const bool first = (tile0 == 0 && tid == 0);
+	/* the very first record of the text has no delimiter in front of it: thread 0 of tile 0.  (delim_kind 3 in a window after
+	 * the first: the start rows do not hold the delimiter's state there, and that record belongs to the window before) */
+	const bool first = (tile0 == 0 && tid == 0) && (C.kind != 3 || P.own_lo == INT64_MIN);
 	uint32_t owned = first ? 1u : 0u;
 #pragma unroll
 	for (int w = 0; w < DENSE_PER / 64; w++) owned += __popcll(bits[w]);

@@ -53,7 +53,7 @@ extern "C" void agb_shutdown(void)
 		cudaFree(W.tile_counts); cudaFree(W.tile_offsets); cudaFree(W.cand); cudaFree(W.cand_counts); cudaFree(W.cand_offsets);
 		cudaFree(W.cand_first); cudaFree(W.scan_sums); cudaFree(W.scan_offs); cudaFree(W.ord_blocks); cudaFree(W.totals);
 		cudaFreeHost(W.h_totals); cudaFree(W.d_desc); cudaFree(W.d_gram); cudaFreeHost(W.h_gram);
-		cudaFree(W.d_regex);
+		cudaFree(W.d_regex); cudaFree(W.ds_func); cudaFree(W.ds_entry); cudaFree(W.dstate);
 		if (W.e0) cudaEventDestroy(W.e0); if (W.e1) cudaEventDestroy(W.e1); if (W.e2) cudaEventDestroy(W.e2);
 		W = Workspace();
 	}
@@ -227,9 +227,12 @@ static int records_launch(const agb_desc &d, Workspace &W, const void *d_text, u
 	P.records = d_records; P.capacity = capacity;
 	P.totals = W.totals; P.emit = 0; P.levels = (want & AGB_WANT_LEVELS) ? 1 : 0; P.want_level = want_level;
 	P.own_lo = sh ? sh->own_lo : INT64_MIN; P.own_hi = sh ? sh->own_hi : INT64_MAX; P.shard_last = sh ? sh->last : 1;
-	P.rx_tab = W.d_regex; P.rx_tail = W.regex_tail;
+	P.rx_tab = W.d_regex; P.rx_tail = W.regex_tail; P.dstate = W.dstate;
 	if (!n) return AGB_OK;
 	const bool want_list = (want & AGB_WANT_RECORDS) && capacity;
+	/* (delim_kind 3 has no anchor plan: only the dense tile form reads the delimiter pass, the other forms find record
+	 * starts by the delimiter's bytes) */
+	if (d.delim_kind == 3 && (in != REC_EVERY_BYTE || slices_usable(d))) { snprintf(g_err, sizeof g_err, "internal: delim_kind 3 outside the dense tile form"); return AGB_ERR_ARG; }
 	if (d.engine == AGB_ENGINE_REGEX)
 		return tile_stage(launch_regex, d, P, W, (unsigned)((n + RX_TILE - 1) / RX_TILE), want_list, st);
 	if (in == REC_SURVIVORS) {
@@ -509,6 +512,7 @@ static int stages_after_front(const agb_desc &d, Workspace &W, const void *d_tex
 {
 	int rc;
 	const uint64_t n_chunks = (n + 15) / 16;
+	if (d.delim_kind == 3) { rc = dstate_launch(d, W, d_text, n, sh ? sh->dseed : -1, st); if (rc) return rc; }
 	RecInput in = use_front ? REC_FRONT : REC_EVERY_BYTE;
 	if (in == REC_FRONT && refine_cannot_thin(d)) { bool dense = false; rc = front_is_dense(W, n, st, &dense); if (rc) return rc; if (dense) in = REC_EVERY_BYTE; }
 	if (in == REC_FRONT) { bool refined = false; rc = refine_launch(d, W, d_text, n, st, &refined); if (rc) return rc; if (refined) in = REC_SURVIVORS; }
@@ -896,6 +900,7 @@ static int scan_windowed(const agb_desc &d, const agb_pattern *px, SliceSource &
 	rc = upload(H, src, 0, win_geom(n, w, 0, AGB_HALO_LEFT, AGB_HALO_RIGHT).hi, B.buf[0], WIN_SLACK); if (rc) return rc;
 	CUDA_TRY(cudaStreamSynchronize(H.s_copy));
 	uint64_t copied = 0; long long origin = 0, closes_before = 0;
+	int dseed = -1, next_dseed = -1;                         /* delim_kind 3: the delimiter's state in front of a window's scan */
 	for (uint64_t i = 0; i < m; i++) {
 		/* the next window on its way while this one is scanned (the thread has the pinned ring and src.dfd to itself until joined) */
 		int up_rc = AGB_OK; char up_err[sizeof g_err] = "";
@@ -918,11 +923,14 @@ static int scan_windowed(const agb_desc &d, const agb_pattern *px, SliceSource &
 		uint64_t hl = AGB_HALO_LEFT, hr = AGB_HALO_RIGHT;
 		const uint8_t *base = B.buf[i & 1];
 		WinGeom g; agb_result lres; agb_shard_part part;
+		/* delim_kind 3: the next window's scan starts where this one determines the delimiter's state (its lo lies inside this
+		 * window's range; a kind-3 left halo is never too short) */
+		const int64_t next_lo = i + 1 < m ? (int64_t)win_geom(n, w, i + 1, AGB_HALO_LEFT, AGB_HALO_RIGHT).lo : -1;
 		for (;;) {
 			g = win_geom(n, w, i, hl, hr);
 			const uint64_t room = want_list ? std::min<uint64_t>(capacity - copied, B.rec_cap / sizeof(agb_record)) : 0;
 			rc = shard_window_scan(d, px, base + g.hl, g.n_local, g.hl, g.hr, g.first, g.open_end, g.reaches_end, want,
-			                       B.rec, room, H.s_comp, &lres, &part);
+			                       B.rec, room, H.s_comp, &lres, &part, dseed, next_lo >= 0 ? next_lo - (int64_t)g.lo : -1, &next_dseed);
 			if (rc < 0) return rc;
 			int short_halos = rc;
 			if (g.lo == 0) short_halos &= ~HALO_SHORT_LEFT;      /* the scan starts where the text does: a run there really begins there */
@@ -960,6 +968,7 @@ static int scan_windowed(const agb_desc &d, const agb_pattern *px, SliceSource &
 			copied += lres.n_records;
 		}
 		if (ord) { closes_before += (long long)part.closes; res->n_closes += part.closes; }
+		dseed = next_dseed;
 		rc = join_up(); if (rc) return rc;
 	}
 	res->n_records = copied;
@@ -1146,6 +1155,9 @@ extern "C" int agb_scan_set(const agb_pattern *p, const void *const *h_texts, co
 	P.own_lo = INT64_MIN; P.own_hi = INT64_MAX; P.shard_last = 1;
 	P.rx_tab = W.d_regex; P.rx_tail = W.regex_tail;
 	P.set_files = d_files; P.set_tiles = d_rtiles; P.set_stats = d_stats;
+	/* -p with a delimiter of two or more bytes: the delimiter's state over the ordinals tiles, every file from its own start */
+	if (d.delim_kind == 3) { rc = dstate_launch(d, W, H.text, bytes, -1, H.s_comp, d_files, d_otiles, otiles.size()); if (rc) return rc; }
+	P.dstate = W.dstate;
 	if (!rtiles.empty()) {
 		rc = tile_stage(d.engine == AGB_ENGINE_REGEX ? launch_regex_set : launch_dense_set, d, P, W, (unsigned)rtiles.size(), want_list, H.s_comp);
 		if (rc) return rc;

@@ -107,6 +107,9 @@ struct RecParams {
 	const void *rx_tab; int rx_tail;
 	/* a set of files (agb_scan_set, the kernels' SET form): block b scans tile set_tiles[b].tile of file set_tiles[b].file */
 	const struct SetFile *set_files; const struct SetTile *set_tiles; unsigned long long *set_stats;
+	/* delim_kind 3: the delimiter's state at the start of every 128-byte slice (delim_state.cu; a set: slice 256 t + i of its
+	 * ordinals tile t, SetFile.ord_tile0) */
+	const uint8_t *dstate;
 };
 /* agb_scan_set: file f is the text [off, off + n) of one device buffer (off a multiple of 16), scanned as if alone.  A tile of
  * the record stage (32 KiB) and of the ordinals (32 KiB of [0, n + L)) lies in one file, so a block of the SET form takes its
@@ -116,7 +119,8 @@ struct RecParams {
 struct SetFile { uint64_t off, n; uint32_t ord_tile0; int32_t j0; };
 struct SetTile { uint32_t file, tile; };
 #define SET_STATS 16
-struct ShardInfo { int64_t own_lo, own_hi; int last; };
+/* dseed: delim_kind 3, the delimiter's state in front of the scanned bytes (-1: the text's own start, the virtual '\n') */
+struct ShardInfo { int64_t own_lo, own_hi; int last; int dseed; };
 #define DENSE_THREADS 256
 #define DENSE_TILE    32768
 #define RX_TILE       32768                               /* regex.cu: k_regex's tile */
@@ -148,6 +152,7 @@ struct OrdParams {
 	agb_record *records; const unsigned long long *totals; uint64_t capacity;
 	uint8_t delim[AGB_MAXDELIM + 2], dfold[AGB_MAXDELIM + 2]; int L, kind;   /* delim: folded (lower case where dfold is 0x20) */
 	long long j0;                /* 0, or -1 when the text starts with the user's delimiter (bitap.c:151-156) */
+	const uint8_t *dstate;       /* delim_kind 3: as RecParams.dstate */
 };
 
 /* does the record opened by the delimiter that starts at `begin` belong to this scan (see RecParams.own_lo)?
@@ -195,6 +200,8 @@ struct Workspace {               /* grow-only device scratch, one per device */
 	int sm_count = 0;
 	/* the Next tables of the last regular expression scanned (regex.cu), and their host copy */
 	uint64_t *d_regex = nullptr; uint64_t h_regex[8 * 256]; size_t regex_bytes = 0; int regex_tail = 0;
+	/* delim_kind 3 (delim_state.cu): per 32 KiB tile its transition function and entry state, per 128-byte slice its entry state */
+	uint32_t *ds_func = nullptr; uint8_t *ds_entry = nullptr, *dstate = nullptr; size_t ds_tiles = 0;
 };
 
 /* scan.cu */
@@ -207,11 +214,13 @@ int  scan_device_impl(const agb_desc &d, const void *d_text, uint64_t n, int wan
 /* px (here and below): the pattern that holds what its descriptor cannot -- a regular expression's follow sets, the words
  * of 320-bit rows; NULL for a descriptor that needs neither */
 /* shard.cu: one window of the windowed scan -- the shard scan, with a halo that is too short reported as a positive code
- * (a set of HALO_SHORT_*) instead of an error; and the window's records made global on the device */
+ * (a set of HALO_SHORT_*) instead of an error; and the window's records made global on the device.  delim_kind 3: dseed is
+ * the delimiter's state in front of the scanned range, *state_out gets its state at offset state_at of that range */
 enum { HALO_SHORT_RIGHT = 1, HALO_SHORT_LEFT = 2 };
 int  shard_window_scan(const agb_desc &d, const agb_pattern *px, const void *d_win, uint64_t n_local, uint64_t halo_left, uint64_t halo_right,
                        bool first, bool open_end, bool reaches_end, int want, agb_record *d_records, uint64_t capacity,
-                       cudaStream_t st, agb_result *lres, agb_shard_part *part);
+                       cudaStream_t st, agb_result *lres, agb_shard_part *part,
+                       int dseed = -1, int64_t state_at = -1, int *state_out = nullptr);
 int  shard_window_rebase(agb_record *d_records, uint64_t n, long long byte_add, long long ord_add, bool ordinals, cudaStream_t st);
 /* front.cu */
 bool front_usable(const agb_desc &d);
@@ -239,6 +248,10 @@ bool slices_usable(const agb_desc &d);
 /* regex.cu: stage 2 of AGB_ENGINE_REGEX (RecParams.rx_tab set), and its tables (returns the bytes written: 32- or 64-bit words) */
 int  launch_regex(const agb_desc &d, const RecParams &P, unsigned grid, cudaStream_t st);
 size_t regex_tables(const agb_desc &d, const agb_regex &rx, uint64_t *out);
+/* delim_state.cu: the delimiter's state at every slice of [0, n + L) into W.dstate (delim_kind 3); seed: the state in front
+ * of the text (-1: after the virtual '\n'); a set: the slices of its ordinals tiles, each file from the virtual '\n' */
+int  dstate_launch(const agb_desc &d, Workspace &W, const void *d_text, uint64_t n, int seed, cudaStream_t st,
+                   const struct SetFile *set_files = nullptr, const struct SetTile *set_tiles = nullptr, uint64_t set_n_tiles = 0);
 /* aux.cu */
 __global__ void k_gram_sample(const uint8_t *text, uint64_t n_chunks, uint32_t nblk, uint32_t blk_chunks,
                               int ngram, const uint32_t *gram, const uint32_t *gmask, uint32_t fold, unsigned int *counts,

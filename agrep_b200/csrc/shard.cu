@@ -248,7 +248,7 @@ static int comm_buffers(agb_comm *c, uint64_t local_cap, uint64_t pad_cap)
 static int shard_scan_geom(const agb_desc &d, const void *d_shard, uint64_t n_local, uint64_t halo_left, uint64_t halo_right,
                            bool first, bool open_end, bool reaches_end, int want, int want_level,
                            agb_record *d_records, uint64_t capacity, cudaStream_t st, agb_result *lres, agb_shard_part *part,
-                           const agb_pattern *px = nullptr, bool grow = false)
+                           const agb_pattern *px = nullptr, bool grow = false, int dseed = -1, int64_t state_at = -1, int *state_out = nullptr)
 {
 	if (((uintptr_t)d_shard & 15) || (halo_left & 15)) { snprintf(g_err, sizeof g_err, "shard pointer and left halo must be 16-byte aligned"); return AGB_ERR_ARG; }
 	if ((!first && (halo_left % 512)) || (!open_end && ((halo_left + n_local) % 512))) { snprintf(g_err, sizeof g_err, "shard boundaries must fall on multiples of 512 bytes of the scanned range"); return AGB_ERR_ARG; }
@@ -258,6 +258,7 @@ static int shard_scan_geom(const agb_desc &d, const void *d_shard, uint64_t n_lo
 	sh.own_lo = first ? INT64_MIN : (int64_t)halo_left;
 	sh.own_hi = open_end ? INT64_MAX : (int64_t)(halo_left + n_local);
 	sh.last = reaches_end ? 1 : 0;
+	sh.dseed = dseed;
 	int rc = scan_device_impl(d, text, n, want, want_level, d_records, (want & AGB_WANT_RECORDS) ? capacity : 0, st, lres, &sh, px);
 	if (rc) return rc;
 	memset(part, 0, sizeof *part);
@@ -267,6 +268,13 @@ static int shard_scan_geom(const agb_desc &d, const void *d_shard, uint64_t n_lo
 	std::lock_guard<std::mutex> lk(g_ws_mu[dev]);
 	Workspace &W = g_ws[dev];
 	const bool ord = (want & AGB_WANT_ORDINALS) != 0;
+	if (state_out && d.delim_kind == 3 && state_at >= 0) {
+		/* the delimiter's state at state_at (a multiple of 512) of the scanned range: where the next window's scan starts */
+		uint8_t *h = reinterpret_cast<uint8_t *>(W.h_totals + 19);
+		CUDA_TRY(cudaMemcpyAsync(h, W.dstate + state_at / 128, 1, cudaMemcpyDeviceToHost, st));
+		CUDA_TRY(cudaStreamSynchronize(st));
+		*state_out = *h;
+	}
 	const int short_halos = (W.h_totals[11] ? HALO_SHORT_RIGHT : 0) | (W.h_totals[18] ? HALO_SHORT_LEFT : 0);
 	if (!grow && W.h_totals[11]) { snprintf(g_err, sizeof g_err, "a record of this shard runs past its halo (%d bytes behind the shard)", AGB_HALO_RIGHT); return AGB_ERR_ARG; }
 	if (!grow && W.h_totals[18]) { snprintf(g_err, sizeof g_err, "a run of the delimiter longer than the left halo (%llu bytes) crosses the start of this shard", (unsigned long long)halo_left); return AGB_ERR_ARG; }
@@ -287,10 +295,20 @@ static int shard_scan_geom(const agb_desc &d, const void *d_shard, uint64_t n_lo
  * global on the device -- begin/end += byte_add, ordinal += ord_add -- by the gather kernel over a world of one */
 int shard_window_scan(const agb_desc &d, const agb_pattern *px, const void *d_win, uint64_t n_local, uint64_t halo_left, uint64_t halo_right,
                       bool first, bool open_end, bool reaches_end, int want, agb_record *d_records, uint64_t capacity,
-                      cudaStream_t st, agb_result *lres, agb_shard_part *part)
+                      cudaStream_t st, agb_result *lres, agb_shard_part *part, int dseed, int64_t state_at, int *state_out)
 {
 	return shard_scan_geom(d, d_win, n_local, halo_left, halo_right, first, open_end, reaches_end, want, -1, d_records, capacity, st,
-	                       lres, part, px, true);
+	                       lres, part, px, true, dseed, state_at, state_out);
+}
+
+/* the sharded scans cannot give a rank the delimiter's state at the start of its shard (the halos are too short for it) */
+static int refuse_sticky(const agb_desc &d, char *err = nullptr, size_t errlen = 0)
+{
+	if (d.delim_kind != 3) return AGB_OK;
+	const char *msg = "-p with a delimiter of more than one byte is not supported by the sharded scans (a shard's records depend on all the text before it)";
+	snprintf(g_err, sizeof g_err, "%s", msg);
+	if (err && errlen) snprintf(err, errlen, "%s", msg);
+	return AGB_ERR_PATTERN;
 }
 
 int shard_window_rebase(agb_record *d_records, uint64_t n, long long byte_add, long long ord_add, bool ordinals, cudaStream_t st)
@@ -310,6 +328,7 @@ extern "C" int agb_scan_shard_local(const agb_pattern *p, const void *d_shard, u
 {
 	if (!p || !res || !part) return AGB_ERR_ARG;
 	if ((want & AGB_WANT_RECORDS) && capacity && !d_records) return AGB_ERR_ARG;
+	if (refuse_sticky(p->d)) return AGB_ERR_PATTERN;
 	return shard_scan_geom(p->d, d_shard, n_local, halo_left, halo_right, first != 0, open_end != 0, reaches_end != 0, want, -1,
 	                       d_records, capacity, (cudaStream_t)stream, res, part, p);
 }
@@ -396,6 +415,7 @@ extern "C" int agb_scan_sharded(const agb_pattern *p, agb_comm *c, const void *d
 {
 	if (!p || !c || !res) return AGB_ERR_ARG;
 	if ((want & AGB_WANT_RECORDS) && capacity && !d_records) return AGB_ERR_ARG;
+	if (refuse_sticky(p->d)) return AGB_ERR_PATTERN;
 	cudaStream_t st = (cudaStream_t)stream;
 	CUDA_TRY(cudaSetDevice(c->dev));
 	agb_result lres;
@@ -421,6 +441,7 @@ extern "C" int agb_bestmatch_sharded(const char *pattern, const agb_options *opt
 	o.bestmatch = 1; o.k = 0;
 	*best_k = -1;
 	int rc = agbi_build(pattern, &o, &d, err, errlen); if (rc) return rc;
+	if (refuse_sticky(d, err, errlen)) return AGB_ERR_PATTERN;
 	int kmax = d.M - 1; if (kmax > AGB_MAXERR) kmax = AGB_MAXERR; if (kmax > m - 1) kmax = m - 1;
 	const int want = AGB_WANT_LEVELS | (capacity ? AGB_WANT_RECORDS : AGB_WANT_COUNT);
 	const int stages[3] = { 2, 4, 8 }; int prev = -1;

@@ -52,6 +52,9 @@ typedef struct agb_options {
 	const char *delim;    /* -d  argument as typed, NULL = newline records                   */
 	int32_t wide_approx;  /* 1: accept a simple literal of 64 to AGB_WIDE_MAXPOS positions at k = 1..8 (what the
 	                         reference's sgrep() takes, up to 255 characters) in 320-bit rows; 0: refuse it     */
+	int32_t sticky_delim; /* 1: accept -p (Init1 = ~0) with a delimiter of 2..AGB_MAXDELIM bytes, whose positions are then
+	                         sticky too, so that records close at the delimiter as a subsequence (delim_kind 3);
+	                         0: refuse it                                                                       */
 } agb_options;
 
 /* engines = which reference function the descriptor stands for */
@@ -76,7 +79,9 @@ typedef struct agb_desc {
 	int32_t  start_closes;    /* 1: the virtual '\n' closes a (never reported) record, scan starts from reset[] */
 	int32_t  M, L;            /* positions; delimiter length                                  */
 	uint8_t  delim[2 * AGB_MAXDELIM + 2];
-	int32_t  delim_kind;      /* 0: border-free (every occurrence closes a record); 1: c^L run rule */
+	int32_t  delim_kind;      /* 0: border-free (every occurrence closes a record); 1: c^L run rule; 2: a self-overlapping
+	                             delimiter (taken from the left); 3: -p with L >= 2, the delimiter's positions sticky: the
+	                             closes come from a scan of the delimiter's state over the text (DESIGN 3.3.1) */
 	int32_t  k;               /* error rows                                                   */
 	int32_t  nrows;           /* k+1, or 2k+1 for ASEARCH1 (rows k..2k live)                  */
 	int32_t  cost_i, cost_s, cost_d;
@@ -108,6 +113,10 @@ typedef struct agb_desc {
 	/* 1: the automaton's rows are 320 bits wide and its words are in agb_pattern_wide(), not here (set by agb_compile only;
 	 * 0 from every caller) */
 	uint8_t  wide;
+	/* 1: the caller accepts delim_kind 3 (-p with a delimiter of two or more bytes): set by agb_compile when
+	 * agb_options.sticky_delim is on and the pattern needs it, by the caller of agb_pattern_from_desc; 0 refuses such
+	 * a descriptor */
+	uint8_t  sticky_delim;
 } agb_desc;
 
 typedef struct agb_pattern agb_pattern;       /* opaque: agb_desc + bookkeeping              */
@@ -289,6 +298,8 @@ int  agb_scan_sharded(const agb_pattern *p, agb_comm *c, const void *d_shard, ui
  *   begin/end += byte_base + (offset of the shard in the whole text);
  *   ordinal   += ord_origin of the first shard + the closes of all shards before this one - ord_fix. */
 typedef struct agb_shard_part { uint64_t closes; int64_t ord_fix, ord_origin, byte_base; int32_t virt, pad; } agb_shard_part;
+/* The sharded scans refuse a pattern of delim_kind 3 with AGB_ERR_PATTERN: a rank would need the delimiter's state at
+ * the start of its shard, which the halos cannot give. */
 int  agb_scan_shard_local(const agb_pattern *p, const void *d_shard, uint64_t n_local, uint64_t halo_left, uint64_t halo_right,
                           int first, int open_end, int reaches_end, int want, agb_record *d_records, uint64_t capacity,
                           void *stream, agb_result *res, agb_shard_part *part);
